@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- the warping hot path on B200, measured the way BASELINE.json asks.
+"""bench.py -- the warping hot path on H100, measured the way BASELINE.json asks.
 
     python bench.py [--gpus N] [--steps K] [--warmup W]          our CUDA path
+    python bench.py ... --dump-outputs DIR                        also write the last timed step's outputs as .npy
     python bench.py --impl reference [...]                        the reference's CPU path
 
 Workload (BASELINE.json configs[1], the configuration the metric is quoted on):
@@ -19,7 +20,8 @@ Printed JSON (one line, rank 0):
              H2D of source/flow/logits/grad_out and D2H of out + the three gradients
              inside the timed region
   roofline   dominant kernel of the step: algorithmic bytes / CUDA-event duration vs
-             the measured HBM peak (MEASURED_PEAKS.json); roofline_fwd: the fused forward
+             the HBM peak (MEASURED_PEAKS.json if present, else the H100 SXM data sheet's
+             3350 GB/s); roofline_fwd: the fused forward
   cpu_baseline  the reference's own kernel bodies on the host cores (oracle/_ref),
              bounded sample, rank 0 / N=1 only
 """
@@ -59,11 +61,11 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -183,6 +185,25 @@ def cpu_reference_run(steps, warmup, flow_kind="smooth", rows=REF_ROWS):
                       f"{steps} steps (+{warmup} warm-up), unfused reference pipeline; threads = best of {{1, 8, 32, {ncpu // 2}, {ncpu}}} on an 8-row probe"}, sec
 
 
+DUMP_MAX_ELEMS = 1 << 22     # per array: 4 outputs x 16 MB of float32 stay under 64 MB
+
+
+def dump_outputs(torch, outdir, result):
+    """The last timed step's outputs in the logical [B, C, H, W] (NCHW) element order, as float32 .npy files.  Arrays larger
+    than DUMP_MAX_ELEMS are sampled at the same seeded element indices on every run (drawn with replacement, repeats dropped,
+    ascending), so two builds compare output for output."""
+    import numpy as np
+    os.makedirs(outdir, exist_ok=True)
+    out, (gs, gf, gl) = result
+    for name, t in (("out", out), ("grad_source", gs), ("grad_flow", gf), ("grad_logits", gl)):
+        flat = t.detach().contiguous().reshape(-1)
+        if flat.numel() > DUMP_MAX_ELEMS:
+            g = torch.Generator(device="cpu").manual_seed(20240611)
+            idx = torch.randint(0, flat.numel(), (DUMP_MAX_ELEMS,), generator=g).unique()
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(outdir, name + ".npy"), flat.float().cpu().numpy())
+
+
 def bind_to_gpu_numa_node(torch, local_rank):
     """pin this process (and so its pinned host buffers, first-touch) to the NUMA node the GPU hangs off"""
     try:
@@ -224,7 +245,7 @@ def extras(torch, F_, dev, args, peak, peak_kind):
       cfg3            BASELINE config 3: resample2d fwd+bwd, B=32 C=128 512x512 fp32, kernel_size 2 (module default) and 4
                       (what training uses), each with its own HBM roofline (1036 / 1560 algorithmic B per pixel, SURVEY.md 8d)
       f4_resample_cosine   the fused resample2d -> cosine op vs the unfused modules (SURVEY row f4), fwd+bwd
-      reference_cuda  the reference's own CUDA kernels recompiled for sm_100a (oracle/_ref/libgfla_ref_cuda.so), running the
+      reference_cuda  the reference's own CUDA kernels recompiled for sm_90a (oracle/_ref/libgfla_ref_cuda.so), running the
                       unfused ExtractorAttn tail in fp32 on 2 samples of the cfg2 shape -- the same-box GPU baseline"""
     out = {}
     B, C, H, W, k = (CFG[x] for x in "BCHWk")
@@ -306,7 +327,7 @@ def extras(torch, F_, dev, args, peak, peak_kind):
         s32, l32, g32 = src.float(), logits.float(), gout.float()
         ms = _time(torch, lambda: rc.local_attn_fwd_bwd(s32, flow, l32, g32, k, chunk=1), 1, 2)
         out["reference_cuda"] = {"value": nb * H * W / (ms * 1e-3) / 1e6, "unit": UNIT, "ms_per_sample": ms / nb, "dtype": "f32",
-                                 "kind": "reference CUDA kernels (block_extractor / local_attn_reshape) recompiled for sm_100a + torch softmax/mul/avg_pool",
+                                 "kind": "reference CUDA kernels (block_extractor / local_attn_reshape) recompiled for sm_90a + torch softmax/mul/avg_pool",
                                  "sample": f"{nb} samples of the cfg2 shape (C={C} {H}x{W} k={k}), fwd+bwd, one sample per launch (the reference's int n limit)"}
     except Exception as exc:
         out["reference_cuda"] = {"unavailable": repr(exc)[:200]}
@@ -332,8 +353,13 @@ def main():
     ap.add_argument("--arms", default="fused,literal,refcuda", help="cfg4/cfg5: comma list, first = the reported value")
     ap.add_argument("--no-extras", action="store_true", help="skip the extra keys (iid flow, cfg3 resample2d, reference CUDA kernels)")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="cfg2: after the timed steps write what the last one computed (out, grad_source, grad_flow, grad_logits) "
+                         "as DIR/<name>.npy in float32; tensors above 4 Mi elements as a fixed, seeded sample")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "cfg2" or args.impl != "ours"):
+        ap.error("--dump-outputs writes the outputs of the cfg2 GPU step only (--workload cfg2 --impl ours)")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -343,7 +369,7 @@ def main():
               "per_gpu_batch": B, "global_batch": B * world, "C": C, "H": H, "W": W, "k": k,
               "flow": args.flow, "layout": "channels_last (NHWC storage)" if args.layout == "nhwc" else "contiguous NCHW",
               "sharding": f"batch x{world} (no data-path collective)",
-              "l2": "inputs (>=1 GiB per step) exceed the 126 MB L2; no explicit flush"}
+              "l2": "inputs (>=1 GiB per step) exceed the 50 MB L2; no explicit flush"}
 
     if args.workload != "cfg2":
         if args.impl == "reference":
@@ -421,11 +447,18 @@ def main():
     barrier()
     t_wall0 = time.time()
     launches0 = _lib.lib().gfla_debug_launch_count()
+    last = None
     for i in range(steps):
-        step(ev[i])
+        res = step(ev[i])
+        if i == steps - 1:
+            last = res          # only the last step's outputs are kept alive, and only after that step was enqueued
+        del res
     launches = int(_lib.lib().gfla_debug_launch_count() - launches0)   # kernels of libgfla_warp.so launched in the timed region
     barrier()
     t_wall1 = time.time()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(torch, args.dump_outputs, last)
+    del last
     total_ms = ev[0][0].elapsed_time(ev[-1][2])
     fwd_ms = sum(e[0].elapsed_time(e[1]) for e in ev) / steps
     bwd_ms = sum(e[1].elapsed_time(e[2]) for e in ev) / steps
@@ -445,7 +478,7 @@ def main():
             step_planar()
         barrier()
         a_, b__ = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        p_steps = max(steps, 20)
+        p_steps = steps
         a_.record()
         for _ in range(p_steps):
             step_planar()
@@ -520,26 +553,15 @@ def main():
     peak, peak_kind = measured_peak_gbs()
     fwd_bytes, bwd_bytes = algorithmic_bytes(B, C, H, W, k)
 
-    # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` captures
-    # (profiles/traffic.json; cold-cache single launch at this exact workload), or null
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    except Exception:
-        traffic = {}
-
-    def roof(nbytes, ms, kernel, tkey=None):
+    def roof(nbytes, ms, kernel):
         ach = nbytes / (ms * 1e-3) / 1e9
         return {"bound": "hbm", "kernel": kernel, "achieved": ach, "peak": peak, "peak_source": peak_kind, "unit": "GB/s",
-                "frac": ach / peak, "traffic": traffic.get(tkey) if args.layout == "nhwc" and args.flow == "smooth" else None,
-                "algorithmic_bytes": nbytes, "launch_ms": ms}
+                "frac": ach / peak, "algorithmic_bytes": nbytes, "launch_ms": ms}
 
-    rf_fwd = roof(fwd_bytes, fwd_ms, "k_local_attn_fwd_strip (fused forward)", "fwd")
-    fused_bwd = os.environ.get("GFLA_BWD_FUSED", "1") != "0"
-    rf_bwd = roof(bwd_bytes, bwd_ms, "k_local_attn_bwd_fused (fused backward, zero fill of grad_source inside the kernel)" if fused_bwd
-                  else "k_local_attn_bwd_gs_tc + k_local_attn_bwd_q_tc + grad_source memset", "bwd")
+    rf_fwd = roof(fwd_bytes, fwd_ms, "k_local_attn_fwd_tc (fused forward)")
+    rf_bwd = roof(bwd_bytes, bwd_ms, "grad_source memset + k_local_attn_bwd_tc (fused backward)")
     rf_fwd["share_of_step"], rf_bwd["share_of_step"] = fwd_ms / ms_per_step, bwd_ms / ms_per_step
-    # The step is two launches: the fused forward (~1/3 of the time) and the fused backward (~2/3; ncu launch list:
-    # profiles/r2_bench_launches.md).  `roofline` describes the DOMINANT one by measured share; both are always reported.
+    # `roofline` describes the DOMINANT part of the step by measured share; both are always reported.
     dominant = dict(rf_bwd if bwd_ms >= fwd_ms else rf_fwd)
     line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": steps, "warmup": warmup,
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,

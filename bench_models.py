@@ -9,7 +9,7 @@ Constructor arguments are the task models' (pose_model.py:62-64, face_model.py:7
 Arms (what sits under `ExtractorAttn`, base_function.py:790-818):
   fused    this package's ExtractorAttn: conv logits + ONE fused local-attention kernel (the product path)
   literal  the reference's ExtractorAttn class, unchanged, on this package's unfused BlockExtractor / LocalAttnReshape
-  refcuda  the reference's ExtractorAttn class on the reference's own CUDA kernels recompiled for sm_100a
+  refcuda  the reference's ExtractorAttn class on the reference's own CUDA kernels recompiled for sm_90a
            (oracle/_ref/libgfla_ref_cuda.so) -- the "patched reference ops" baseline of SURVEY.md section 8(d)
 
 cfg4  PoseGenerator forward + backward under DistributedDataParallel (NCCL gradient all-reduce -- the only collective

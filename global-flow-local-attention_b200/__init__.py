@@ -1,4 +1,6 @@
-"""gfla_b200 -- B200-native (sm_100a) warping hot path of Global-Flow-Local-Attention.
+"""gfla_b200 -- H100-native (sm_90a) warping hot path of Global-Flow-Local-Attention.
+
+The package keeps its historical name ``gfla_b200``.
 
 The directory is called ``global-flow-local-attention_b200`` (not an importable
 name), so the repo root carries ``gfla_b200.py`` which loads it under the module

@@ -55,7 +55,7 @@ def lib() -> ctypes.CDLL:
         if not os.path.exists(LIB_PATH):
             raise GflaError(
                 f"{LIB_PATH} is not built. Run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). There is no CPU / PyTorch fallback for these ops.")
+                "(nvcc, sm_90a). There is no CPU / PyTorch fallback for these ops.")
         l = ctypes.CDLL(LIB_PATH)
         for name, argtypes in SIGNATURES.items():
             fn = getattr(l, name)          # AttributeError if the .so lacks a declared symbol

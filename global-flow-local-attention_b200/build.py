@@ -1,11 +1,9 @@
-"""Build libgfla_warp.so (sm_100a only) in-tree with nvcc.
+"""Build libgfla_warp.so (sm_90a, H100) in-tree with nvcc.
 
     python -m gfla_b200.build          (or  __graft_entry__.build())
 
 The library is a plain C-ABI shared object (include/gfla_warp.h): it does not
-link against torch or libcuda (the driver entry point needed for TMA
-descriptors is fetched at run time through the CUDA runtime), so it
-cross-compiles on a box without a GPU and travels to the GPU box as a file.
+link against torch or libcuda, so it cross-compiles on a machine without a GPU.
 """
 from __future__ import annotations
 
@@ -23,7 +21,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libgfla_warp.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-I", INCLUDE]
 # per-file extras: the unfused ops keep IEEE mul/add separate so that their fp32 /
 # fp64 forward is bit-identical to the (uncontracted) CPU oracle.
@@ -34,7 +32,7 @@ def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError("nvcc not found (needed to build libgfla_warp.so for sm_100a)")
+    raise RuntimeError("nvcc not found (needed to build libgfla_warp.so for sm_90a)")
 
 
 def _digest(paths) -> str:
@@ -57,8 +55,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         path = os.path.join(CSRC, src)
         obj = os.path.join(OBJ, src[:-3] + ".o")
         stamp = obj + ".sha"
-        flags = ARCH + COMMON + EXTRA.get(src, []) + (["-DGFLA_TC_PROFILE"] if os.environ.get("GFLA_BUILD_PROFILE") == "1" else []) + (["-DGFLA_TC_KNOBS_ON"] if os.environ.get("GFLA_BUILD_KNOBS") == "1" else []) \
-            + ([f"-DGFLA_TC_WAIT_CYCLES={int(os.environ['GFLA_TC_WAIT_CYCLES'])}LL"] if os.environ.get("GFLA_TC_WAIT_CYCLES") else [])
+        flags = ARCH + COMMON + EXTRA.get(src, [])
         dig = _digest([path] + headers) + " " + " ".join(flags)
         if not force and os.path.exists(obj) and os.path.exists(stamp) and open(stamp).read() == dig:
             continue

@@ -15,24 +15,14 @@ int resample2d_cos_bwd(const void*, const void*, const void*, const void*, const
                        int, int, int, double, int, int, cudaStream_t);
 int local_attn_fwd_gather(const void*, const void*, const void*, void*, void*, const void*, const void*, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
 int local_attn_bwd_gather(const void*, const void*, const void*, const void*, void*, void*, void*, int, int, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
-bool local_attn_bwd_tc_supported(int C, int k, int dtype, int flow_dtype, int layout, const void* gout, const void* gsrc);
-bool local_attn_bwd_q_tc_supported(int C, int k);
-int local_attn_bwd_q_tc(const void* src, const void* flow, const void* logits, const void* gout, void* gflow, void* glogits, int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate, cudaStream_t);
-bool local_attn_bwd_fused_supported(int C, int k, const void* src);
-int local_attn_bwd_fused_tc(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow, void* glogits, int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate, void* workspace, long long workspace_bytes, cudaStream_t);
-int local_attn_bwd_gs_tc(const void* flow, const void* logits, const void* gout, void* gsrc, int B, int C, int Hs, int Ws, int H, int W, int k, cudaStream_t);
+bool local_attn_bwd_tc_supported(int C, int k, int dtype, int flow_dtype, int layout, const void* src, const void* gout, const void* gsrc);
+int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow, void* glogits, int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate, cudaStream_t);
 int local_attn_fwd_tc(const void*, const void*, const void*, void*, void*, const void*, const void*, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
 int relayout(const void*, void*, int, int, int, int, int, int, cudaStream_t);
-int tc_debug_set_buffer(void*);
-int tc_debug_set_buffer_bwd(void*);
-int tc_wait_profile_fwd(int, unsigned long long*);
-int tc_wait_profile_strip(int, unsigned long long*);
-int tc_wait_profile_bwd_fused(int, unsigned long long*);
 bool local_attn_fwd_tc_supported(int B, int C, int Hs, int Ws, int H, int W, int k, int dtype, int flow_dtype, int layout, const void* src, const void* out);
 }  // namespace gfla
 
 #include <atomic>
-#include <cstdlib>
 
 namespace gfla {
 static std::atomic<unsigned long long> g_launches{0};
@@ -40,9 +30,6 @@ void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 }  // namespace gfla
 
 using namespace gfla;
-
-// which backward the automatic path takes where both can serve the call (GFLA_BWD_FUSED=0/1 overrides)
-constexpr bool kBwdFusedDefault = true;
 
 #define REQ_PTR(p) do { if ((p) == nullptr) return GFLA_E_NULL; } while (0)
 #define REQ_ALIGN(p, dt) do { if (!aligned((p), elem_size(dt))) return GFLA_E_ALIGN; } while (0)
@@ -72,22 +59,20 @@ int gfla_device_check(void) {
     if (e != cudaSuccess) return static_cast<int>(e);
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-    return (major == 10 && minor == 0) ? GFLA_OK : static_cast<int>(cudaErrorNoKernelImageForDevice);
+    return (major == 9 && minor == 0) ? GFLA_OK : static_cast<int>(cudaErrorNoKernelImageForDevice);
 }
 
+// The tile kernels keep no wait profile and no debug channel; the entry points stay for ABI compatibility.
 int gfla_debug_wait_profile(int which, int enable, unsigned long long* out_u64x64) {
-    if (which < 0 || which > 2) return GFLA_E_SHAPE;
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) return static_cast<int>(e);
-    if (which == 2) return tc_wait_profile_bwd_fused(enable, out_u64x64);
-    return which == 0 ? tc_wait_profile_fwd(enable, out_u64x64) : tc_wait_profile_strip(enable, out_u64x64);
+    (void)enable; (void)out_u64x64;
+    return (which < 0 || which > 2) ? GFLA_E_SHAPE : GFLA_E_NOTSUP;
 }
 
 unsigned long long gfla_debug_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
 int gfla_debug_set_buffer(void* host_mapped_u64x8) {
-    const int e = tc_debug_set_buffer(host_mapped_u64x8);
-    return e ? e : tc_debug_set_buffer_bwd(host_mapped_u64x8);
+    (void)host_mapped_u64x8;
+    return GFLA_E_NOTSUP;
 }
 
 int gfla_relayout(const void* src, void* dst, int B, int C, int H, int W, int dtype, int to_nhwc, gfla_stream_t stream) {
@@ -237,55 +222,12 @@ static int local_attn_bwd_any(const void* source, const void* flow, const void* 
     if (algo < 0 || algo > 2) return GFLA_E_NOTSUP;
     REQ_ALIGN(source, dtype); REQ_ALIGN(logits, dtype); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_source, dtype);
     REQ_ALIGN(grad_logits, dtype); REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
-    const bool tc_ok = local_attn_bwd_tc_supported(C, k, dtype, flow_dtype, layout, grad_out, grad_source);
+    const bool tc_ok = local_attn_bwd_tc_supported(C, k, dtype, flow_dtype, layout, source, grad_out, grad_source);
     if (algo == 2 && !tc_ok) return GFLA_E_NOTSUP;
-    if (algo == 2 || (algo == 0 && tc_ok)) {
-        // grad_source: tile kernel (GEMM + TMA reduce-add); grad_flow / grad_logits: per-pixel dot products.
-        // The batch is walked in chunks of `cb` samples (zero-fill, grad_source kernel, grad_flow/logits kernel per chunk):
-        // with a chunk's grad_source + grad_out + source (3 * C*H*W*2 bytes per sample) inside the 126 MB L2, the zero-fill
-        // never reaches HBM before the reduce-adds land on it, and the second kernel finds grad_out still in L2.
-        const size_t per_s = (size_t)C * Hs * Ws * elem_size(dtype), per_o = (size_t)C * H * W * elem_size(dtype);
-        const size_t per_f = (size_t)2 * H * W * elem_size(flow_dtype), per_l = (size_t)k * k * H * W * elem_size(dtype);
-        int cb = B;
-        {
-            const char* v = getenv("GFLA_BWD_CHUNK");
-            if (v) cb = atoi(v) > 0 ? atoi(v) : B;
-        }
-        const bool q_tc = local_attn_bwd_q_tc_supported(C, k);
-        // one fused kernel (grad_out tile read once) where it can serve the shape; GFLA_BWD_FUSED=0 keeps the two-kernel path
-        bool fused = kBwdFusedDefault && local_attn_bwd_fused_supported(C, k, source);
-        {
-            const char* v = getenv("GFLA_BWD_FUSED");
-            if (v) fused = atoi(v) != 0 && local_attn_bwd_fused_supported(C, k, source);
-        }
-        for (int b0 = 0; b0 < B; b0 += cb) {
-            const int nb = (B - b0 < cb) ? (B - b0) : cb;
-            const char* s_ = (const char*)source + b0 * per_s;
-            const char* f_ = (const char*)flow + b0 * per_f;
-            const char* l_ = (const char*)logits + b0 * per_l;
-            const char* g_ = (const char*)grad_out + b0 * per_o;
-            char* gs_ = (char*)grad_source + b0 * per_s;
-            char* gf_ = (char*)grad_flow + b0 * per_f;
-            char* gl_ = (char*)grad_logits + b0 * per_l;
-            int e = GFLA_OK;
-            if (fused) {
-                e = local_attn_bwd_fused_tc(s_, f_, l_, g_, gs_, gf_, gl_, nb, C, Hs, Ws, H, W, k, accumulate, workspace, workspace_bytes,
-                                            (cudaStream_t)stream);
-                if (e != GFLA_OK) return e;
-                continue;
-            }
-            if (!accumulate) e = zero_async(gs_, nb * per_s, (cudaStream_t)stream);
-            if (e == GFLA_OK) e = local_attn_bwd_gs_tc(f_, l_, g_, gs_, nb, C, Hs, Ws, H, W, k, (cudaStream_t)stream);
-            if (e != GFLA_OK) return e;
-            if (q_tc)
-                e = local_attn_bwd_q_tc(s_, f_, l_, g_, gf_, gl_, nb, C, Hs, Ws, H, W, k, accumulate, (cudaStream_t)stream);
-            else
-                e = local_attn_bwd_gather(s_, f_, l_, g_, gs_, gf_, gl_, nb, C, Hs, Ws, H, W, k, dtype, flow_dtype, accumulate,
-                                          layout, /*do_gs=*/0, (cudaStream_t)stream);
-            if (e != GFLA_OK) return e;
-        }
-        return GFLA_OK;
-    }
+    (void)workspace; (void)workspace_bytes;
+    if (algo == 2 || (algo == 0 && tc_ok))
+        return local_attn_bwd_tc(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, accumulate,
+                                 (cudaStream_t)stream);
     return local_attn_bwd_gather(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W,
                                  k, dtype, flow_dtype, accumulate, layout, /*do_gs=*/1, (cudaStream_t)stream);
 }
@@ -297,7 +239,7 @@ int gfla_local_attn_bwd(const void* source, const void* flow, const void* logits
                               flow_dtype, layout, accumulate, algo, nullptr, 0, stream);
 }
 
-long long gfla_local_attn_bwd_workspace_bytes(int B) { return B > 0 ? 4LL * B + 4LL * 4096 : 0; }   // counters per sample + a progress word per CTA (<= SM count)
+long long gfla_local_attn_bwd_workspace_bytes(int B) { (void)B; return 0; }   // the tile backward needs no workspace
 
 int gfla_local_attn_bwd_ws(const void* source, const void* flow, const void* logits, const void* grad_out,
                            void* grad_source, void* grad_flow, void* grad_logits, int B, int C, int Hs, int Ws, int H, int W,

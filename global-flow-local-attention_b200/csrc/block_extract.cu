@@ -1,4 +1,4 @@
-// block_extractor and local_attn_reshape for sm_100a (CUDA-core kernels).
+// block_extractor and local_attn_reshape for sm_90a (CUDA-core kernels).
 //
 // What they compute is fixed by the reference
 // (block_extractor/block_extractor_kernel.cu:20-170,

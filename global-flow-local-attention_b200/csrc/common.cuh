@@ -1,4 +1,4 @@
-// Shared device/host helpers for the GFLA warping library (sm_100a only).
+// Shared device/host helpers for the GFLA warping library (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

@@ -10,8 +10,8 @@
 // never materialised.
 //
 // These kernels serve every dtype / k / shape (they are what fp32, fp64 and
-// small or odd shapes run on, and the general fall-back of the tcgen05 tile
-// kernel in local_attn_tc.cu).  One thread owns one output pixel:
+// small or odd shapes run on: everything the tensor-core tile kernels in
+// local_attn_tc.cu / local_attn_bwd_tc.cu do not serve).  One thread owns one output pixel:
 //   * softmax over the k*k logits in registers (coalesced plane-strided loads);
 //   * when the k taps along each axis are consecutive integers (always, except
 //     when fp32 rounding of (flow+offset)+coord straddles an integer) the

@@ -1,4 +1,4 @@
-// resample2d (Gaussian-weighted ks x ks warp, FlowNet2-derived) for sm_100a.
+// resample2d (Gaussian-weighted ks x ks warp, FlowNet2-derived) for sm_90a.
 //
 // Arithmetic contract: resample2d_package/resample2d_kernel.cu:20-95 (forward),
 // :98-202 (grad input1), :204-330 (grad input2 = d/d(dx, dy, sigma)).
@@ -15,13 +15,9 @@
 //     tap offsets live in registers and are reused for every channel;
 //     a CTA owns a 32 x 4 pixel tile: a warp is a 128-byte
 //     row segment, and the ks rows a pixel row reads are shared with the rows
-//     above / below through L1 (one-row CTAs pulled every source row ks times
-//     over the L2 -> L1 fabric: 6.4x the tensor, profiles/r2_resample2d.md);
+//     above / below through L1 instead of each row being pulled over the L2 -> L1 fabric ks times;
 //     channel slices in grid.y for small images;
 //   * grad_input1: warps whose taps are one integer shift of their pixel run merge the scatter through shuffles.
-//     (Measured and dropped, profiles/r2_resample2d.md: accumulating the CTA's scatter in a shared-memory box and
-//     flushing the box -- fp32 shared-memory atomics are ATOMS.CAST.SPIN loops, 2.6 tries and 7 wavefronts per
-//     add on a stretching flow, no faster than the L2's native fp32 RED.)
 //   * grad_input2: the reference runs 3*H*W threads that each stride twice
 //     through all C channel planes; here one thread per pixel accumulates the
 //     4*(ks/2)^2 corner dot products sum_c g[c]*v[c,corner] in ONE pass and

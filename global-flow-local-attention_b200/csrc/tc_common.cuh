@@ -1,8 +1,7 @@
-// sm_100a building blocks shared by the tcgen05 tile kernels: mbarrier, TMA,
-// TMEM allocation, UMMA descriptors.  Raw PTX (no CUTLASS dependency); bit
-// layouts follow the PTX ISA tcgen05 descriptor definitions.
+// sm_90a building blocks shared by the tensor-core tile kernels: cp.async staging, ldmatrix fragment loads and
+// the warp-level bf16 MMA (m16n8k16, fp32 accumulate).  Raw PTX, no CUTLASS dependency.
 #pragma once
-#include <cuda.h>  // CUtensorMap & enums only -- the driver entry point is fetched at run time
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -13,98 +12,6 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
-// ------------------------------------------------------------------ mbarrier
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-// Debug channel: a host-mapped (pinned) buffer of 8 x u64 set through gfla_debug_set_buffer(); survives a trap.
-static __device__ unsigned long long* g_tc_dbg = nullptr;
-
-// Bounded wait: a protocol bug must abort the kernel (trap -> launch error), never hang the GPU.  The bound is a
-// safety net, not a scheduling assumption: ~10 s of SM cycles by default (time-slicing, MPS preemption, a
-// debugger or compute-sanitizer can legitimately stretch a wait by orders of magnitude over the ~microseconds a
-// healthy pipeline needs); build with -DGFLA_TC_WAIT_CYCLES=<n> for a shorter fuse while developing a kernel.
-// `tag` identifies the waiter (role << 16 | barrier kind << 8 | slot) in the debug buffer.
-#ifndef GFLA_TC_WAIT_CYCLES
-#define GFLA_TC_WAIT_CYCLES 20000000000LL
-#endif
-static __device__ __noinline__ __attribute__((noreturn)) void mbar_timeout(uint32_t tag, uint32_t parity, uint32_t iter) {
-    unsigned long long* d = g_tc_dbg;
-    if (d != nullptr) {
-        if (atomicCAS(d, 0ull, (unsigned long long)tag | (1ull << 63)) == 0ull) {
-            d[1] = parity; d[2] = iter; d[3] = blockIdx.x; d[4] = threadIdx.x;
-        }
-        __threadfence_system();
-    }
-    __trap();
-    __builtin_unreachable();     // noreturn: no wait site has to keep its registers alive across this call
-}
-// Wait profile (debug builds only: GFLA_BUILD_PROFILE=1 python build.py, i.e. -DGFLA_TC_PROFILE): cycles that
-// lane 0 of every warp spent blocked, per (role, barrier kind) of the tag, plus explicit region timers (kinds 6, 7);
-// slot 7 of role 0 = total kernel cycles summed over the CTAs.  8 roles x 8 kinds = 64 counters.  Read through gfla_debug_wait_profile().
-#ifdef GFLA_TC_PROFILE
-static __device__ unsigned long long g_tc_prof[64];
-static __device__ int g_tc_prof_on = 0;
-__device__ __forceinline__ void tc_profile_add(int role, int kind, long long cycles) {   // call from every lane or lane 0
-    // always on in profile builds (the host API only resets / reads the counters): testing a global "enabled" flag here put a
-    // global load in front of every barrier wait and made the profiled kernel 2.4x slower than the one it is meant to explain
-    if ((threadIdx.x & 31) == 0) atomicAdd(&g_tc_prof[role * 8 + kind], static_cast<unsigned long long>(cycles));
-}
-__device__ __forceinline__ long long tc_profile_clock() { return clock64(); }
-inline int tc_wait_profile(int enable, unsigned long long* out64) {
-    cudaError_t e = cudaSuccess;
-    if (out64 != nullptr) e = cudaMemcpyFromSymbol(out64, g_tc_prof, sizeof(unsigned long long) * 64);
-    if (e == cudaSuccess) {
-        const unsigned long long zero[64] = {};
-        e = cudaMemcpyToSymbol(g_tc_prof, zero, sizeof(zero));
-    }
-    if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_tc_prof_on, &enable, sizeof(int));
-    return static_cast<int>(e);
-}
-#else
-__device__ __forceinline__ void tc_profile_add(int, int, long long) {}
-__device__ __forceinline__ long long tc_profile_clock() { return 0; }
-inline int tc_wait_profile(int, unsigned long long*) { return GFLA_E_NOTSUP; }
-#endif
-__device__ __forceinline__ void tc_profile_total(long long t_start) {
-    if (threadIdx.x == 0) tc_profile_add(0, 7, tc_profile_clock() - t_start);
-}
-
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32_t tag = 0, uint32_t iter = 0) {
-#ifdef GFLA_TC_PROFILE
-    const long long t0 = clock64();
-    while (!mbar_try_wait(bar, parity)) {   // try_wait itself suspends the thread for a while before giving up
-        if (clock64() - t0 > GFLA_TC_WAIT_CYCLES) mbar_timeout(tag, parity, iter);
-    }
-    const long long dt = clock64() - t0;
-    if (dt > 64) tc_profile_add((tag >> 16) & 7, (tag >> 8) & 7, dt);
-#else
-    if (mbar_try_wait(bar, parity)) return;
-    const long long t0 = clock64();
-    while (!mbar_try_wait(bar, parity)) {
-        if (clock64() - t0 > GFLA_TC_WAIT_CYCLES) mbar_timeout(tag, parity, iter);
-    }
-#endif
-}
-
 // explicit shared-space accesses (32-bit shared addresses): keeps ptxas from falling back to generic LD/ST
 __device__ __forceinline__ void sts128(uint32_t a, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
@@ -113,87 +20,45 @@ __device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st
 __device__ __forceinline__ void sts16(uint32_t a, uint32_t v) {
     asm volatile("{\n\t.reg .b16 h;\n\tcvt.u16.u32 h, %1;\n\tst.shared.b16 [%0], h;\n\t}" ::"r"(a), "r"(v) : "memory");
 }
-__device__ __forceinline__ void lds128(uint32_t a, float& x, float& y, float& z, float& w) {
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(x), "=f"(y), "=f"(z), "=f"(w) : "r"(a) : "memory");
-}
-__device__ __forceinline__ uint32_t lds32(uint32_t a) {
-    uint32_t v;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+__device__ __forceinline__ void stsf(uint32_t a, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); }
+__device__ __forceinline__ float ldsf(uint32_t a) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a) : "memory");
     return v;
 }
 
-// 32-byte streaming global store (sm_100 256-bit STG): one full sector per lane instead of two half-sector writes
-__device__ __forceinline__ void stg256_cs(void* gptr, const uint32_t (&w)[8]) {
-    asm volatile("st.global.cs.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(gptr), "r"(w[0]), "r"(w[1]), "r"(w[2]),
-                 "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
+// ------------------------------------------------------------------ cp.async (global -> shared, 16 bytes)
+// src_bytes = 0 zero-fills the destination without reading global memory
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes = 16) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05 operand reads)
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// ------------------------------------------------------------------ TMA
-__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
+// ------------------------------------------------------------------ ldmatrix / mma
+// four 8x8 b16 matrices; lane l supplies the row address of matrix l/8
+__device__ __forceinline__ void ldsm_x4(uint32_t a, uint32_t (&r)[4]) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a) : "memory");
 }
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
+__device__ __forceinline__ void ldsm_x4_t(uint32_t a, uint32_t (&r)[4]) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a) : "memory");
+}
+// D (+)= A[16x16, row] * B[16x8, col], bf16 in, fp32 accumulate (warp-collective)
+__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
+        "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// shared -> global tensor tile store / reduce-add (bulk async-group completion)
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-// L2 eviction-priority policies (createpolicy) and the hinted forms of the copies above
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-__device__ __forceinline__ void tma_load_4d_hint(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3,
-                                                 uint64_t policy) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5, %6}], [%2], %7;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(policy)
-        : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_4d_hint(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2, int c3,
-                                                       uint64_t policy) {
-    asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.bulk_group.L2::cache_hint [%0, {%2, %3, %4, %5}], [%1], %6;"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(policy) : "memory");
-}
-__device__ __forceinline__ void stg128_zero_hint(void* gptr, uint64_t policy) {
-    asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1, %1, %1, %1}, %2;" ::"l"(gptr), "r"(0u), "l"(policy) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>   // at most N of this thread's bulk groups still READING their shared-memory source
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-template <int N>   // at most N of this thread's bulk groups not yet complete (writes performed)
-__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
-
-// L2 prefetch of a contiguous global range (16-byte aligned address and size)
-__device__ __forceinline__ void prefetch_l2_bulk(const void* gptr, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(gptr)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* m, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global [%0, {%1, %2, %3, %4}];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+__device__ __forceinline__ uint32_t bf16_bits(float v) {
+    const __nv_bfloat16 h = __float2bfloat16_rn(v);
+    return static_cast<uint32_t>(*reinterpret_cast<const unsigned short*>(&h));
 }
 
-// Division of tile / group indices by run-time image geometry: magic multiplier computed once per thread at kernel start, then
-// umulhi + shift per use (an integer division is ~25 dependent instructions, and every role decodes its group index per group).
+// Division of group indices by run-time image geometry: magic multiplier computed once, then umulhi + shift per use.
 // Exact for 0 <= n < 2^31, d >= 1.
 struct FastDiv {
     uint32_t d, mul, shr;
@@ -207,100 +72,6 @@ struct FastDiv {
     __device__ __forceinline__ uint32_t div(uint32_t n) const { return d != 1 ? __umulhi(n, mul) >> shr : n; }
     __device__ __forceinline__ void divmod(uint32_t n, uint32_t& q, uint32_t& r) const { q = div(n); r = n - q * d; }
 };
-
-// One lane of a converged warp (the same one every time).  MMA issue must branch on THIS, not on `lane == 0`: after
-// elect.sync the compiler knows a single lane is live and moves descriptors to the uniform registers UTCHMMA wants with
-// one R2UR each; behind a plain lane test it emits a waterfall loop (ELECT / R2UR.BROADCAST / BRA.U.ANY) per operand,
-// ~100 cycles per MMA -- more than a 128x64x16 MMA takes to execute.
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-
-// ------------------------------------------------------------------ TMEM / tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {  // one thread; arrives on `bar` when all prior MMAs retire
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16/f16 inputs, fp32 accumulate; one thread issues
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// the same with the A operand in TMEM (128 lanes x K/2 32-bit columns of packed 16-bit values)
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// shared memory -> TMEM copy of a [128 rows][32 bytes] matrix (same matrix descriptor as an MMA operand); one thread issues,
-// ordered with the tcgen05.mma / tcgen05.cp instructions of the same thread
-__device__ __forceinline__ void tmem_cp_128x256b(uint32_t taddr, uint64_t s_desc) {
-    asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(taddr), "l"(s_desc) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (warp-collective)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------ descriptors
-// Instruction descriptor, kind::f16: c_format[4,6) (1 = F32), a_format[7,10), b_format[10,13) (0 = F16, 1 = BF16),
-// a_major bit 15, b_major bit 16 (0 = K-major, 1 = MN-major), n_dim[17,23) = N>>3, m_dim[24,29) = M>>4.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, bool bf16, bool a_mn_major, bool b_mn_major) {
-    return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | ((a_mn_major ? 1u : 0u) << 15) |
-           ((b_mn_major ? 1u : 0u) << 16) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-// Shared-memory matrix descriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48),
-// base_offset [49,52) = 0, layout [61,64): 0 none, 2 = 128B, 4 = 64B, 6 = 32B swizzle.
-enum : uint64_t { kSwizzleNone = 0, kSwizzle128 = 2, kSwizzle64 = 4, kSwizzle32 = 6 };
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint64_t layout) {
-    return static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4) | (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16) |
-           (static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46) | (layout << 61);
-}
-
-// ------------------------------------------------------------------ host: tensor maps
-typedef CUresult (*PFN_tmapEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                        const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                        CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-inline PFN_tmapEncodeTiled tmap_encoder() {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-        return nullptr;
-    return reinterpret_cast<PFN_tmapEncodeTiled>(fn);
-}
 
 }  // namespace tc
 }  // namespace gfla

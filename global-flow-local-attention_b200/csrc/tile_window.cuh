@@ -1,9 +1,7 @@
 // Pieces shared by the forward and backward tile kernels: pixel-group geometry, per-pixel softmax,
-// the reference's tap arithmetic, the collapsed (k+1)x(k+1) weight window and its scatter into the
-// [128 pixels][16 positions] UMMA weight slabs.
+// the reference's tap arithmetic and the collapsed (k+1)x(k+1) weight window.
 #pragma once
 #include <climits>
-#include <cstdlib>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -12,10 +10,7 @@ namespace gfla {
 namespace tc {
 
 constexpr int GW = 16, GH = 8;          // pixel group: 16 x 8 = 128 pixels (= M or K of the MMAs)
-constexpr int BW = 16;                  // source positions per row segment = 32-byte swizzle span in bf16 = one MMA K
-constexpr int A_SLAB = 128 * 32;        // bytes: [128 pixels][16 positions] bf16, 32B rows, 32B swizzle
-
-struct GroupInfo { int x0, y0, ncb, nrc; };
+constexpr int SEG = 16;                 // source positions per row segment = one MMA K step
 
 // softmax over the KK logits of one pixel (bf16 planes, stride hw), fp32 arithmetic
 template <int KK>
@@ -175,53 +170,6 @@ __device__ __forceinline__ void build_window(const float* p, const AxisTap<float
     }
 }
 
-// window rows as packed bf16x2 words in shared memory: word (r*(K1/2) + q) of pixel m at wsm_a + idx*512
-template <int K>
-__device__ __forceinline__ void store_window_words(uint32_t wsm_a, const float* w) {
-    constexpr int K1 = K + 1;
-#pragma unroll
-    for (int r = 0; r < K1; ++r)
-#pragma unroll
-        for (int q = 0; q < K1 / 2; ++q) {
-            const __nv_bfloat162 v2 = __floats2bfloat162_rn(w[r * K1 + 2 * q], w[r * K1 + 2 * q + 1]);
-            sts32(wsm_a + (r * (K1 / 2) + q) * 512, *reinterpret_cast<const uint32_t*>(&v2));
-        }
-}
-
-// One 32-byte slab row (this pixel x 16 positions of one source row segment): zero it, then drop in the
-// window row r (if the segment holds any of its K+1 columns).  e0 = box position of window column 0.
-// `dirty` remembers (one bit per slab row of the ring, kept by the owning thread) whether the row currently
-// holds non-zero weights: rows that are still all-zero from their last use are not rewritten.
-// Returns true if anything was stored (the caller then needs the async-proxy fence).
-template <int K, int BWT = BW>
-__device__ __forceinline__ bool fill_slab_row(uint32_t row, uint32_t swz, uint32_t wsm_a, bool hit, int r, int e0,
-                                              uint32_t& dirty, uint32_t bit) {
-    constexpr int K1 = K + 1;
-    const bool write = hit && r >= 0 && r <= K;
-    if (!write && !(dirty & bit)) return false;
-    // zero the whole row; the 16-byte chunks go out in swizzled order: with rows of 64 (32) bytes, lanes 0, 2, 4, ... (0, 4, 8, ...)
-    // would otherwise hit the same 4 banks with the same chunk -- a 4-way conflict on every one of these stores, and they
-    // were 2/3 of all shared-memory store wavefronts of the forward kernel (ncu: l1tex__data_bank_conflicts_pipe_lsu_mem_shared_op_st)
-#pragma unroll
-    for (int ch = 0; ch < BWT / 8; ++ch) sts128(row + ((ch * 16) ^ swz), 0u, 0u, 0u, 0u);
-    dirty &= ~bit;
-    if (write) {
-        dirty |= bit;
-        uint32_t wv[K1 / 2];
-#pragma unroll
-        for (int q = 0; q < K1 / 2; ++q) wv[q] = lds32(wsm_a + (r * (K1 / 2) + q) * 512);
-#pragma unroll
-        for (int c = 0; c < K1; ++c) {
-            const int e = e0 + c;
-            if (e >= 0 && e < BWT) {
-                const uint32_t half = (c & 1) ? (wv[c >> 1] >> 16) : (wv[c >> 1] & 0xffffu);
-                sts16(row + ((((e >> 3) << 4) ^ swz)) + (e & 7) * 2, half);   // swz = swizzle XOR of this row's 16B chunks
-            }
-        }
-    }
-    return true;
-}
-
 // One "irregular" pixel (taps not consecutive integers: fp32 rounding of (flow+offset)+coord straddling an integer,
 // ~1e-5 of all pixels) with the reference's literal 4-taps-per-(i,j) arithmetic (block_extractor_kernel.cu:57-82
 // followed by base_function.py:804-810).  One such pixel costs 4*k*k*CN dependent loads, so a whole warp shares it:
@@ -265,22 +213,6 @@ __device__ __forceinline__ void irregular_pixel(const __nv_bfloat16* __restrict_
         }
         ob[NHWC ? (long long)c : (long long)c * hw] = __float2bfloat16_rn(acc);
     }
-}
-
-// Ablation switches of the tile kernels (GFLA_TC_KNOBS / GFLA_BWD_KNOBS, read per launch) exist only in a tuning build
-// (GFLA_BUILD_KNOBS=1 python build.py, i.e. -DGFLA_TC_KNOBS_ON).  The shipped kernels compile them out: the ~20 extra
-// branches cost the fused backward 12 % (0.99 -> 1.11 ms measured when four more were added, profiles/r2_l2_policy.md) --
-// these kernels run 6 role programs on one SM and are sensitive to code size.
-#ifdef GFLA_TC_KNOBS_ON
-#define GFLA_KNOBS(k) (k)
-#else
-#define GFLA_KNOBS(k) 0
-#endif
-
-// tuning knobs (environment, read per launch)
-inline int tune_knob(const char* name, int dflt) {
-    const char* v = getenv(name);
-    return v ? atoi(v) : dflt;
 }
 
 }  // namespace tc

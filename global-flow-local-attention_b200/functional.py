@@ -28,7 +28,7 @@ def _need_cuda(*ts: torch.Tensor) -> None:
     for t in ts:
         if not t.is_cuda:
             # same behaviour as the reference ops: there is no CPU implementation
-            raise NotImplementedError("GFLA warp ops are CUDA-only (sm_100a); got a CPU tensor")
+            raise NotImplementedError("GFLA warp ops are CUDA-only (sm_90a); got a CPU tensor")
     dev = ts[0].device
     for t in ts:
         if t.device != dev:
@@ -274,7 +274,7 @@ def local_attn_bwd(source, flow, logits, grad_out, k, algo="auto"):
     _need_cuda(source, flow, logits, grad_out)
     if (layout == _lib.GFLA_NCHW and algo == "auto" and _tile_bwd_eligible(source, flow, k)
             and not source.is_contiguous(memory_format=torch.channels_last)):   # H=W=1 / C=1: both formats at once
-        # The backward tile kernels are channels-last only (every operand must be channel-contiguous for TMA).
+        # The backward tile kernel is channels-last only (every operand is staged as channel-contiguous 16-byte chunks).
         # For planar callers, re-lay the two feature tensors (two extra passes over them) instead of falling
         # back to the scalar-atomics kernel: ~100x faster at cfg2.
         go = grad_out if grad_out.is_contiguous() else grad_out.contiguous()
@@ -282,14 +282,18 @@ def local_attn_bwd(source, flow, logits, grad_out, k, algo="auto"):
         return relayout(gs, False), gf, gl
     fmt = torch.channels_last if layout == _lib.GFLA_NHWC else torch.contiguous_format
     grad_out = grad_out.contiguous(memory_format=fmt)
+    tile = layout == _lib.GFLA_NHWC and _tile_bwd_eligible(source, flow, k)
+    if source.dtype in (torch.bfloat16, torch.float16) and (algo == "gather" or (algo == "auto" and not tile)):
+        # The CUDA-core backward scatters grad_source with one atomic add per (pixel, tap, channel).  In a 16-bit type every
+        # add rounds, and the order-dependent rounding of up to (k+1)^2 adds per element exceeds the bf16 tolerance: run it
+        # on fp32 copies and round each gradient once.
+        gs, gf, gl = local_attn_bwd(source.float(), flow.float(), logits.float(), grad_out.float(), k, algo="gather")
+        return gs.to(source.dtype), gf.to(flow.dtype), gl.to(logits.dtype)
     bs, ds, hs, ws = source.size()
     _, _, h, w = flow.size()
     gs, gf, gl = _like_layout(source, source.shape, layout), torch.empty_like(flow), torch.empty_like(logits)
     with torch.cuda.device_of(source):
-        # scratch for the fused kernel's in-kernel zero-fill of grad_source (per-sample counters; the library never allocates)
-        nws = int(_lib.lib().gfla_local_attn_bwd_workspace_bytes(bs))
-        wsb = torch.empty(max(nws, 4), dtype=torch.uint8, device=source.device)
-        _lib.check(_lib.lib().gfla_local_attn_bwd_ws(_p(source), _p(flow), _p(logits), _p(grad_out), _p(gs), _p(gf), _p(gl),
-                                                     bs, ds, hs, ws, h, w, k, _dt(source), _dt(flow), layout, 0, ALGO[algo],
-                                                     _p(wsb), nws, _stream(source)), "local_attn_bwd")
+        _lib.check(_lib.lib().gfla_local_attn_bwd(_p(source), _p(flow), _p(logits), _p(grad_out), _p(gs), _p(gf), _p(gl),
+                                                  bs, ds, hs, ws, h, w, k, _dt(source), _dt(flow), layout, 0, ALGO[algo],
+                                                  _stream(source)), "local_attn_bwd")
     return gs, gf, gl

@@ -1,5 +1,5 @@
 /*
- * gfla_warp.h -- C ABI of the B200-native (sm_100a) GFLA warping library.
+ * gfla_warp.h -- C ABI of the H100-native (sm_90a) GFLA warping library.
  *
  * This is the drop-in boundary for the warping hot path of
  * RenYurui/Global-Flow-Local-Attention: the three custom extensions under
@@ -66,14 +66,12 @@ enum gfla_error {
 int gfla_abi_version(void);
 /* static string for any code returned by this library (GFLA_E_* or cudaError_t) */
 const char* gfla_error_string(int code);
-/* compute capability the library was built for (100) and whether the running
- * device can execute it; returns 0 when usable. */
+/* whether the running device can execute the library (built for compute capability 9.0, sm_90a);
+ * returns 0 when usable. */
 int gfla_device_check(void);
 
-/* Debug aid for the tile kernels: `host_mapped_u64x8` is a DEVICE-visible pointer to 8
- * zero-initialised uint64 in pinned host memory (or NULL to disable).  If a pipeline
- * barrier inside a tile kernel ever times out, the kernel records which one there and
- * traps instead of hanging the GPU.  Not used on the normal path. */
+/* Former debug channel of the pipelined tile kernels.  The current kernels have no pipeline barriers that could
+ * time out: returns GFLA_E_NOTSUP and does nothing. */
 int gfla_debug_set_buffer(void* host_mapped_u64x8);
 
 /* Statistics: number of kernels this library has launched in this process so far (all entry points, all
@@ -81,12 +79,8 @@ int gfla_debug_set_buffer(void* host_mapped_u64x8);
  * its timed region as `gpu_launches`. */
 unsigned long long gfla_debug_launch_count(void);
 
-/* Debug aid for tuning the tile kernels: cycles their warps spent blocked on the pipeline barriers.
- * Only in profile builds of the library (GFLA_BUILD_PROFILE=1 at build time, -DGFLA_TC_PROFILE); a normal build
- * carries no timing code and returns GFLA_E_NOTSUP.  `which`: 0 = per-tile forward kernel, 1 = strip forward kernel,
- * 2 = fused backward kernel.  Copies the 64 counters collected since the last call into `out_u64x64` (HOST memory, may
- * be NULL), clears them and switches collection on (enable = 1) or off (0).  Index = role * 8 + kind (roles and kinds per
- * kernel: tools/wait_profile.py); [7] = kernel cycles summed over the CTAs.  Synchronises the device. */
+/* Former wait profile of the pipelined tile kernels: returns GFLA_E_SHAPE for `which` outside [0, 2] and
+ * GFLA_E_NOTSUP otherwise (the current kernels collect no profile). */
 int gfla_debug_wait_profile(int which, int enable, unsigned long long* out_u64x64);
 
 /* Re-layout of a [B,C,H,W] feature tensor between planar NCHW and channels-last NHWC storage
@@ -194,7 +188,7 @@ int gfla_resample2d_cosine_bwd(const void* in1, const void* in2, const void* tar
  *   `layout`: GFLA_NCHW (the reference's contiguous layout) or GFLA_NHWC (channels-last: every
  *           source position is 2*C contiguous bytes -- the layout the tile kernels are fastest on).
  *   `algo`: 0 = automatic choice, 1 = CUDA-core gather kernel,
- *           2 = tcgen05 tile kernel (GFLA_E_NOTSUP if it cannot serve the call).
+ *           2 = tensor-core tile kernel (GFLA_E_NOTSUP if it cannot serve the call).
  * ------------------------------------------------------------------------ */
 int gfla_local_attn_fwd(const void* source, const void* flow, const void* logits,
                         void* out, void* probs,
@@ -215,12 +209,9 @@ int gfla_local_attn_bwd(const void* source, const void* flow, const void* logits
                         int B, int C, int Hs, int Ws, int H, int W, int k,
                         int dtype, int flow_dtype, int layout, int accumulate, int algo,
                         gfla_stream_t stream);
-/* The same backward with a caller-provided scratch buffer (DEVICE memory, >= gfla_local_attn_bwd_workspace_bytes(B) bytes,
- * 4-byte aligned, contents irrelevant, may be reused by the next call on the same stream).  With it -- and accumulate = 0 --
- * the fused tcgen05 backward zero-fills grad_source INSIDE the kernel, sample by sample just ahead of its own reduce-adds
- * (per-sample completion counters live in the workspace), instead of a separate memset pass in front of it: one pass less
- * over the 2*C*Hs*Ws*B bytes, and the zeros are still in L2 when the adds land on them.  workspace = NULL behaves exactly
- * like gfla_local_attn_bwd.  The library itself never allocates. */
+/* The same backward with a caller-provided scratch buffer (DEVICE memory, >= gfla_local_attn_bwd_workspace_bytes(B) bytes).
+ * The current kernels need no scratch: the size is 0, the buffer is ignored and the call behaves exactly like
+ * gfla_local_attn_bwd.  Kept so that callers written against ABI version 1 keep linking. */
 long long gfla_local_attn_bwd_workspace_bytes(int B);
 int gfla_local_attn_bwd_ws(const void* source, const void* flow, const void* logits,
                            const void* grad_out,

@@ -34,7 +34,7 @@ def build(ref: bool | None = None) -> None:
         subprocess.check_call(["make", "-s", "-C", _HERE, "ref"])
         import shutil
         if shutil.which("nvcc") or os.path.exists("/usr/local/cuda/bin/nvcc"):
-            # the same extracted text through nvcc (sm_100a): GPU-side oracle + "reference CUDA kernels, recompiled" baseline
+            # the same extracted text through nvcc (sm_90a): GPU-side oracle + "reference CUDA kernels, recompiled" baseline
             subprocess.check_call(["make", "-s", "-C", _HERE, "refcuda"])
 
 

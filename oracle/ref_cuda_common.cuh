@@ -1,6 +1,6 @@
 /*
  * TEST INFRASTRUCTURE ONLY.
- * Launch helpers for the reference's CUDA kernel bodies compiled for sm_100a (oracle/_ref/libgfla_ref_cuda.so):
+ * Launch helpers for the reference's CUDA kernel bodies compiled for sm_90a (oracle/_ref/libgfla_ref_cuda.so):
  * the same extracted text as the host build (oracle/Makefile), this time through nvcc, behind plain
  * extern "C" launchers that take device pointers -- no ATen.  Geometry = the reference launchers'
  * <<<ceil(n/256), 256, 0, stream>>> with `int n` (block_extractor_kernel.cu:172-217, 222-278;

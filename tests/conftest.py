@@ -12,16 +12,18 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 def load_golden(name):
-    """-> {case: {key: array}} from tests/golden/<name>.npz"""
-    z = np.load(os.path.join(GOLDEN, name + ".npz"))
+    """-> {case: {key: array}} from tests/golden/<name>.npz and its parts <name>.<case>.npz (files stay under 1 MB)"""
     cases = {}
-    for full in z.files:
-        case, key = full.split("/", 1)
-        cases.setdefault(case, {})[key] = z[full]
+    for f in sorted(os.listdir(GOLDEN)):
+        if f == name + ".npz" or (f.startswith(name + ".") and f.endswith(".npz")):
+            z = np.load(os.path.join(GOLDEN, f))
+            for full in z.files:
+                case, key = full.split("/", 1)
+                cases.setdefault(case, {})[key] = z[full]
     return cases
 
 

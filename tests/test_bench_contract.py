@@ -1,5 +1,5 @@
 """bench.py's reference arm runs on the host alone: check the JSON line it prints against the bench contract
-(the GPU arm prints the same keys plus roofline / clocks / gpu_launches; it needs a B200 and is exercised by the driver)."""
+(the GPU arm prints the same keys plus roofline / clocks / gpu_launches; it needs an H100)."""
 import json
 import os
 import subprocess

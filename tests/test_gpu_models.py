@@ -3,8 +3,8 @@ on this library -- BASELINE configs 4 and 5 at test size, SURVEY rows f2/f3.
 
   * one PoseGenerator / FaceGenerator forward with the fused ExtractorAttn equals the literal reference op chain
     (reference ExtractorAttn class on the unfused ops), and -- where the library was built -- the chain on the
-    reference's own CUDA kernels recompiled for sm_100a;
-  * the INTEGRATION.md recipe (`.bfloat16().to(memory_format=channels_last)`) reaches the tcgen05 tile kernels in
+    reference's own CUDA kernels recompiled for sm_90a;
+  * the INTEGRATION.md recipe (`.bfloat16().to(memory_format=channels_last)`) reaches the tensor-core tile kernels in
     forward AND backward (the flow is bf16 there: it is widened to fp32, ADVICE r1);
   * AffineRegularizationLoss on the GPU: the reference class on our CUDA ops vs the op-free rewrite in losses.py.
 """
@@ -103,7 +103,7 @@ def test_face_generator_fused_equals_literal(BM):
 
 
 def test_bf16_channels_last_generator_reaches_the_tile_kernels(BM):
-    """INTEGRATION.md recipe: every ExtractorAttn level must launch the tcgen05 forward AND backward kernels"""
+    """INTEGRATION.md recipe: every ExtractorAttn level must launch the tensor-core forward AND backward kernels"""
     from torch.profiler import ProfilerActivity, profile
     net = _build(BM, "fused", "pose", torch.bfloat16, cl=True)
     x = _pose_inputs(2, torch.bfloat16, torch.channels_last)
@@ -113,13 +113,37 @@ def test_bf16_channels_last_generator_reaches_the_tile_kernels(BM):
         img.float().mean().backward()
         torch.cuda.synchronize()
     names = [e.key for e in prof.key_averages()]
-    fwd = [n for n in names if "k_local_attn_fwd_strip" in n or "k_local_attn_fwd_tc" in n]
-    bwd = [n for n in names if "k_local_attn_bwd" in n and "_tc" in n or "k_local_attn_bwd_fused" in n]
+    fwd = [n for n in names if "k_local_attn_fwd_tc" in n]
+    bwd = [n for n in names if "k_local_attn_bwd_tc" in n]
     slow = [n for n in names if "gfla::k_local_attn_fwd<" in n or "gfla::k_local_attn_bwd<" in n]
     assert fwd and bwd, names
     assert not slow, slow                                    # no fall-back to the CUDA-core gather kernels
     assert torch.isfinite(img.float()).all()
     assert all(p.grad is None or torch.isfinite(p.grad.float()).all() for p in net.parameters())
+
+
+@pytest.mark.parametrize("level", [(256, 32, 3), (128, 64, 5)])
+def test_bf16_channels_last_extractor_attn_reaches_the_tile_kernels(level):
+    """The same recipe on this package's own ExtractorAttn at the attention levels of the pose generator (C, size, k), with
+    the bf16 flow a converted network hands it -- needs no copy of the reference's generator code"""
+    import gfla_b200
+    from torch.profiler import ProfilerActivity, profile
+    C, S, k = level
+    torch.manual_seed(C + k)
+    cl = torch.channels_last
+    m = gfla_b200.ExtractorAttn(C, k, softmax=True).to(DEV).bfloat16().to(memory_format=cl)
+    src = torch.randn(2, C, S, S, device=DEV).bfloat16().contiguous(memory_format=cl).requires_grad_()
+    tgt = torch.randn(2, C, S, S, device=DEV).bfloat16().contiguous(memory_format=cl)
+    flow = (torch.rand(2, 2, S, S, device=DEV) * 6 - 3).bfloat16().requires_grad_()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        out = m(src, tgt, flow)
+        out.float().mean().backward()
+        torch.cuda.synchronize()
+    names = [e.key for e in prof.key_averages()]
+    assert any("k_local_attn_fwd_tc" in n for n in names), names
+    assert any("k_local_attn_bwd_tc" in n for n in names), names
+    assert not [n for n in names if "gfla::k_local_attn_fwd<" in n or "gfla::k_local_attn_bwd<" in n]
+    assert torch.isfinite(out.float()).all() and torch.isfinite(src.grad.float()).all() and torch.isfinite(flow.grad.float()).all()
 
 
 @pytest.mark.parametrize("kz", [3, 5])

@@ -3,7 +3,7 @@
 Two reference builds travel with the snapshot (git-ignored, built by ``__graft_entry__.build()`` where
 /root/reference exists):
   * ``oracle/_ref/libgfla_ref.so``       -- the reference kernel bodies compiled for the host (OpenMP);
-  * ``oracle/_ref/libgfla_ref_cuda.so``  -- the same extracted text compiled by nvcc for sm_100a
+  * ``oracle/_ref/libgfla_ref_cuda.so``  -- the same extracted text compiled by nvcc for sm_90a
     (``oracle/ref_cuda*.cu``: plain launchers, no ATen) = "the reference's CUDA kernels, recompiled".
 The CUDA build reaches BASELINE.json's full sizes in milliseconds, so the `<5,256>` tile instantiations
 that bench.py times are checked here at 256x256, C=256, k=5 -- forward and backward -- against the reference

@@ -1,10 +1,10 @@
 """Per-op timings at BASELINE.json's configurations (CUDA events, warm-up 3, mean of N) -> JSON lines.
-Secondary to bench.py (which carries the headline contract); results are copied into profiles/."""
+Secondary to bench.py (which carries the headline contract)."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from gfla_b200 import functional as F_
-PEAK = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists("MEASURED_PEAKS.json") else 6650.0
+PEAK = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists("MEASURED_PEAKS.json") else 3350.0   # H100 SXM data sheet
 dev = "cuda:0"
 
 def timed(fn, n=5, w=3):
