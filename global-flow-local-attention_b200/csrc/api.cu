@@ -14,12 +14,12 @@ int resample2d_cos_fwd(const void*, const void*, const void*, void*, void*, int,
 int resample2d_cos_bwd(const void*, const void*, const void*, const void*, const void*, void*, void*, void*, void*, int, int, int, int, int,
                        int, int, int, double, int, int, cudaStream_t);
 int local_attn_fwd_gather(const void*, const void*, const void*, void*, void*, const void*, const void*, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
-int local_attn_bwd_gather(const void*, const void*, const void*, const void*, void*, void*, void*, int, int, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
+int local_attn_bwd_gather(const void*, const void*, const void*, const void*, void*, void*, void*, int, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
 bool local_attn_bwd_tc_supported(int C, int k, int dtype, int flow_dtype, int layout, const void* src, const void* gout, const void* gsrc);
 int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow, void* glogits, int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate, cudaStream_t);
 int local_attn_fwd_tc(const void*, const void*, const void*, void*, void*, const void*, const void*, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
 int relayout(const void*, void*, int, int, int, int, int, int, cudaStream_t);
-bool local_attn_fwd_tc_supported(int B, int C, int Hs, int Ws, int H, int W, int k, int dtype, int flow_dtype, int layout, const void* src, const void* out);
+bool local_attn_fwd_tc_supported(int C, int Ws, int k, int dtype, int flow_dtype, int layout, const void* src, const void* out);
 }  // namespace gfla
 
 #include <atomic>
@@ -88,7 +88,7 @@ int gfla_block_extract_fwd(const void* source, const void* flow, void* out, int 
                            int Wf, int k, int dtype, int flow_dtype, gfla_stream_t stream) {
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(out);
     if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(Hf) || !pos(Wf) || k < 1 || k > 9) return GFLA_E_SHAPE;
-    if (!dtype_known(dtype) || !flow_dtype_ok(dtype, flow_dtype)) return GFLA_E_DTYPE;
+    if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
     REQ_ALIGN(source, dtype); REQ_ALIGN(out, dtype); REQ_ALIGN(flow, flow_dtype);
     return block_extract_fwd(source, flow, out, B, C, Hs, Ws, Hf, Wf, k, dtype, flow_dtype, (cudaStream_t)stream);
 }
@@ -98,9 +98,7 @@ int gfla_block_extract_bwd(const void* source, const void* flow, const void* gra
                            int flow_dtype, int grad_source_dtype, int accumulate, gfla_stream_t stream) {
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(grad_out); REQ_PTR(grad_source); REQ_PTR(grad_flow);
     if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(Hf) || !pos(Wf) || k < 1 || k > 9) return GFLA_E_SHAPE;
-    if (!dtype_known(dtype) || !flow_dtype_ok(dtype, flow_dtype)) return GFLA_E_DTYPE;
-    // grad_source is stored in `dtype`, or in fp32 when `dtype` is a 16-bit type
-    if (grad_source_dtype != dtype && !((dtype == GFLA_BF16 || dtype == GFLA_F16) && grad_source_dtype == GFLA_F32)) return GFLA_E_DTYPE;
+    if (!dtypes_ok(dtype, flow_dtype, grad_source_dtype)) return GFLA_E_DTYPE;
     REQ_ALIGN(source, dtype); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_source, grad_source_dtype);
     REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
     return block_extract_bwd(source, flow, grad_out, grad_source, grad_flow, B, C, Hs, Ws, Hf, Wf, k, dtype, flow_dtype,
@@ -183,12 +181,12 @@ static int local_attn_fwd_any(const void* source, const void* flow, const void* 
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(logits); REQ_PTR(out);
     if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
     if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || k < 1 || k > 9) return GFLA_E_SHAPE;
-    if (!dtype_known(dtype) || !flow_dtype_ok(dtype, flow_dtype)) return GFLA_E_DTYPE;
+    if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
     if (algo < 0 || algo > 2) return GFLA_E_NOTSUP;
     REQ_ALIGN(source, dtype); REQ_ALIGN(logits, dtype); REQ_ALIGN(out, dtype); REQ_ALIGN(flow, flow_dtype);
     if (probs) REQ_ALIGN(probs, dtype);
     if (prev) { REQ_ALIGN(prev, dtype); REQ_ALIGN(mask, dtype); }
-    const bool tc_ok = local_attn_fwd_tc_supported(B, C, Hs, Ws, H, W, k, dtype, flow_dtype, layout, source, out) &&
+    const bool tc_ok = local_attn_fwd_tc_supported(C, Ws, k, dtype, flow_dtype, layout, source, out) &&
                        (prev == nullptr || layout == GFLA_NCHW || aligned(prev, 16));
     if (algo == 2 && !tc_ok) return GFLA_E_NOTSUP;
     if (algo == 2 || (algo == 0 && tc_ok))
@@ -211,32 +209,23 @@ int gfla_local_attn_blend_fwd(const void* source, const void* flow, const void* 
                               algo, stream);
 }
 
-static int local_attn_bwd_any(const void* source, const void* flow, const void* logits, const void* grad_out,
-                              void* grad_source, void* grad_flow, void* grad_logits, int B, int C, int Hs, int Ws, int H, int W,
-                              int k, int dtype, int flow_dtype, int layout, int accumulate, int algo, void* workspace,
-                              long long workspace_bytes, gfla_stream_t stream) {
+int gfla_local_attn_bwd(const void* source, const void* flow, const void* logits, const void* grad_out,
+                        void* grad_source, void* grad_flow, void* grad_logits, int B, int C, int Hs, int Ws, int H, int W,
+                        int k, int dtype, int flow_dtype, int layout, int accumulate, int algo, gfla_stream_t stream) {
     if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(logits); REQ_PTR(grad_out); REQ_PTR(grad_source); REQ_PTR(grad_flow); REQ_PTR(grad_logits);
     if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || k < 1 || k > 9) return GFLA_E_SHAPE;
-    if (!dtype_known(dtype) || !flow_dtype_ok(dtype, flow_dtype)) return GFLA_E_DTYPE;
+    if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
     if (algo < 0 || algo > 2) return GFLA_E_NOTSUP;
     REQ_ALIGN(source, dtype); REQ_ALIGN(logits, dtype); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_source, dtype);
     REQ_ALIGN(grad_logits, dtype); REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
     const bool tc_ok = local_attn_bwd_tc_supported(C, k, dtype, flow_dtype, layout, source, grad_out, grad_source);
     if (algo == 2 && !tc_ok) return GFLA_E_NOTSUP;
-    (void)workspace; (void)workspace_bytes;
     if (algo == 2 || (algo == 0 && tc_ok))
         return local_attn_bwd_tc(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, accumulate,
                                  (cudaStream_t)stream);
     return local_attn_bwd_gather(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W,
-                                 k, dtype, flow_dtype, accumulate, layout, /*do_gs=*/1, (cudaStream_t)stream);
-}
-
-int gfla_local_attn_bwd(const void* source, const void* flow, const void* logits, const void* grad_out,
-                        void* grad_source, void* grad_flow, void* grad_logits, int B, int C, int Hs, int Ws, int H, int W,
-                        int k, int dtype, int flow_dtype, int layout, int accumulate, int algo, gfla_stream_t stream) {
-    return local_attn_bwd_any(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype,
-                              flow_dtype, layout, accumulate, algo, nullptr, 0, stream);
+                                 k, dtype, flow_dtype, accumulate, layout, (cudaStream_t)stream);
 }
 
 long long gfla_local_attn_bwd_workspace_bytes(int B) { (void)B; return 0; }   // the tile backward needs no workspace
@@ -246,8 +235,8 @@ int gfla_local_attn_bwd_ws(const void* source, const void* flow, const void* log
                            int k, int dtype, int flow_dtype, int layout, int accumulate, int algo, void* workspace,
                            long long workspace_bytes, gfla_stream_t stream) {
     if (workspace != nullptr && workspace_bytes < 0) return GFLA_E_SHAPE;
-    return local_attn_bwd_any(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype,
-                              flow_dtype, layout, accumulate, algo, workspace, workspace_bytes, stream);
+    return gfla_local_attn_bwd(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype,
+                               flow_dtype, layout, accumulate, algo, stream);
 }
 
 }  // extern "C"

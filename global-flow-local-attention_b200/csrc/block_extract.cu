@@ -171,9 +171,8 @@ static int launch_be_bwd(const void* src, const void* flow, const void* gout, vo
 
 int block_extract_fwd(const void* src, const void* flow, void* out, int B, int C, int Hs, int Ws, int Hf, int Wf,
                       int k, int dtype, int flow_dtype, cudaStream_t st_) {
-    return GFLA_DISPATCH_T(dtype, [&]() -> int {
-        if (flow_dtype == dtype) return launch_be_fwd<T, T>(src, flow, out, B, C, Hs, Ws, Hf, Wf, k, st_);
-        return launch_be_fwd<T, float>(src, flow, out, B, C, Hs, Ws, Hf, Wf, k, st_);
+    return dispatch_dtypes(dtype, flow_dtype, dtype, [&](auto t, auto tf, auto) -> int {
+        return launch_be_fwd<typename decltype(t)::type, typename decltype(tf)::type>(src, flow, out, B, C, Hs, Ws, Hf, Wf, k, st_);
     });
 }
 
@@ -185,13 +184,9 @@ int block_extract_bwd(const void* src, const void* flow, const void* gout, void*
         if (e == GFLA_OK) e = zero_async(gflow, (size_t)B * 2 * Hf * Wf * elem_size(flow_dtype), st_);
         if (e != GFLA_OK) return e;
     }
-    return GFLA_DISPATCH_T(dtype, [&]() -> int {
-        if (gs_dtype != dtype) {   // 16-bit data, fp32 grad_source buffer
-            if (flow_dtype == dtype) return launch_be_bwd<T, T, float>(src, flow, gout, gsrc, gflow, B, C, Hs, Ws, Hf, Wf, k, st_);
-            return launch_be_bwd<T, float, float>(src, flow, gout, gsrc, gflow, B, C, Hs, Ws, Hf, Wf, k, st_);
-        }
-        if (flow_dtype == dtype) return launch_be_bwd<T, T, T>(src, flow, gout, gsrc, gflow, B, C, Hs, Ws, Hf, Wf, k, st_);
-        return launch_be_bwd<T, float, T>(src, flow, gout, gsrc, gflow, B, C, Hs, Ws, Hf, Wf, k, st_);
+    return dispatch_dtypes(dtype, flow_dtype, gs_dtype, [&](auto t, auto tf, auto tg) -> int {
+        return launch_be_bwd<typename decltype(t)::type, typename decltype(tf)::type, typename decltype(tg)::type>(
+            src, flow, gout, gsrc, gflow, B, C, Hs, Ws, Hf, Wf, k, st_);
     });
 }
 

@@ -122,12 +122,32 @@ inline int zero_async(void* p, size_t bytes, cudaStream_t st_) {
         }                                                                      \
     }()
 
-// flow dtype must equal the data dtype for F32/F64; 16-bit data may pair with
-// a 16-bit flow of the same type or an fp32 flow.
-inline bool flow_dtype_ok(int dtype, int flow_dtype) {
-    if (dtype == GFLA_F32 || dtype == GFLA_F64) return flow_dtype == dtype;
-    if (dtype == GFLA_BF16 || dtype == GFLA_F16) return flow_dtype == dtype || flow_dtype == GFLA_F32;
-    return false;
+template <typename T> struct Type { using type = T; };
+
+// The (data, flow, grad_source) dtype combinations the library serves, listed nowhere else.  fp32 and fp64 data take
+// flow and grad_source of their own type; 16-bit data may widen either to fp32.  Only the block_extractor backward
+// offers an fp32 grad_source: every other op passes the data dtype as gs_dtype.  Calls f(Type<T>{}, Type<TF>{},
+// Type<TG>{}) for a listed combination and returns GFLA_E_DTYPE for anything else.
+template <typename F>
+inline int dispatch_dtypes(int dtype, int flow_dtype, int gs_dtype, F&& f) {
+#define GFLA_DTYPES(D, T, FD, TF, GD, TG) \
+    if (dtype == D && flow_dtype == FD && gs_dtype == GD) return f(Type<T>{}, Type<TF>{}, Type<TG>{});
+    GFLA_DTYPES(GFLA_F32, float, GFLA_F32, float, GFLA_F32, float)
+    GFLA_DTYPES(GFLA_F64, double, GFLA_F64, double, GFLA_F64, double)
+    GFLA_DTYPES(GFLA_BF16, __nv_bfloat16, GFLA_BF16, __nv_bfloat16, GFLA_BF16, __nv_bfloat16)
+    GFLA_DTYPES(GFLA_BF16, __nv_bfloat16, GFLA_F32, float, GFLA_BF16, __nv_bfloat16)
+    GFLA_DTYPES(GFLA_BF16, __nv_bfloat16, GFLA_BF16, __nv_bfloat16, GFLA_F32, float)
+    GFLA_DTYPES(GFLA_BF16, __nv_bfloat16, GFLA_F32, float, GFLA_F32, float)
+    GFLA_DTYPES(GFLA_F16, __half, GFLA_F16, __half, GFLA_F16, __half)
+    GFLA_DTYPES(GFLA_F16, __half, GFLA_F32, float, GFLA_F16, __half)
+    GFLA_DTYPES(GFLA_F16, __half, GFLA_F16, __half, GFLA_F32, float)
+    GFLA_DTYPES(GFLA_F16, __half, GFLA_F32, float, GFLA_F32, float)
+#undef GFLA_DTYPES
+    return GFLA_E_DTYPE;
+}
+
+inline bool dtypes_ok(int dtype, int flow_dtype, int gs_dtype) {
+    return dispatch_dtypes(dtype, flow_dtype, gs_dtype, [](auto, auto, auto) { return GFLA_OK; }) == GFLA_OK;
 }
 
 }  // namespace gfla

@@ -18,36 +18,11 @@
 //     4*k*k bilinear taps collapse into a (k+1)x(k+1) window whose weights are
 //     computed once per pixel and reused for every channel;
 //   * otherwise the pixel takes the literal 4-taps-per-(i,j) path.
-#include "common.cuh"
+#include "local_attn_pixel.cuh"
 
 namespace gfla {
 
 constexpr int kMaxK = 9;
-
-template <typename A> __device__ __forceinline__ A fexp(A v);
-template <> __device__ __forceinline__ float fexp<float>(float v) { return expf(v); }
-template <> __device__ __forceinline__ double fexp<double>(double v) { return exp(v); }
-
-// softmax over the KK logits of one pixel (plane stride hw); returns probabilities
-template <typename T, typename A, int KK_>
-__device__ __forceinline__ void pixel_softmax(const T* __restrict__ lg, long long hw, int KK, A* p) {
-    A m = ld(lg);
-    p[0] = m;
-#pragma unroll
-    for (int t = 1; t < (KK_ ? KK_ : KK); ++t) {
-        p[t] = ld(lg + t * hw);
-        m = p[t] > m ? p[t] : m;
-    }
-    A s = static_cast<A>(0);
-#pragma unroll
-    for (int t = 0; t < (KK_ ? KK_ : KK); ++t) {
-        p[t] = fexp<A>(p[t] - m);
-        s += p[t];
-    }
-    const A inv = static_cast<A>(1) / s;
-#pragma unroll
-    for (int t = 0; t < (KK_ ? KK_ : KK); ++t) p[t] *= inv;
-}
 
 // ---------------------------------------------------------------------------
 // forward
@@ -86,15 +61,9 @@ k_local_attn_fwd(const T* __restrict__ src, const TF* __restrict__ flow, const T
     const A mk = prev ? static_cast<A>(ld(mask + (long long)b * hw + pofs)) : static_cast<A>(1);
 
     bool regular = false;
-    if (K > 0) {
-        AxisTap<A> tx[K ? K : 1], ty[K ? K : 1];
-        regular = true;
-#pragma unroll
-        for (int j = 0; j < K; ++j) {
-            tx[j] = axis_tap<A>(flow_x, j - K / 2, x, Ws);
-            ty[j] = axis_tap<A>(flow_y, j - K / 2, y, Hs);
-            regular = regular && (tx[j].fl == tx[0].fl + j) && (ty[j].fl == ty[0].fl + j);
-        }
+    if constexpr (K > 0) {
+        AxisTap<A> tx[K], ty[K];
+        regular = taps_regular<A, K>(flow_x, flow_y, x, y, Hs, Ws, tx, ty);
         if (regular) {
             constexpr int K1 = K + 1;
             // collapsed window: row r <-> unclamped source row Y0 + r, clamped on use
@@ -136,12 +105,7 @@ k_local_attn_fwd(const T* __restrict__ src, const TF* __restrict__ flow, const T
                 const AxisTap<A> ty = axis_tap<A>(flow_y, i - k / 2, y, Hs);
                 for (int j = 0; j < k; ++j) {
                     const AxisTap<A> tx = axis_tap<A>(flow_x, j - k / 2, x, Ws);
-                    A v = static_cast<A>(0);
-                    v += tx.wlo * ty.wlo * ld(s + (ty.lo * Ws + tx.lo) * sp);
-                    v += tx.whi * ty.wlo * ld(s + (ty.lo * Ws + tx.hi) * sp);
-                    v += tx.wlo * ty.whi * ld(s + (ty.hi * Ws + tx.lo) * sp);
-                    v += tx.whi * ty.whi * ld(s + (ty.hi * Ws + tx.hi) * sp);
-                    acc += p[i * k + j] * v;
+                    acc += p[i * k + j] * tap_value(s, tx, ty, Ws, sp);
                 }
             }
             acc *= inv_kk;
@@ -164,7 +128,7 @@ template <typename T, typename TF, int K>
 __global__ void __launch_bounds__(128)
 k_local_attn_bwd(const T* __restrict__ src, const TF* __restrict__ flow, const T* __restrict__ logits,
                  const T* __restrict__ gout, T* __restrict__ gsrc, TF* __restrict__ gflow, T* __restrict__ glogits,
-                 int B, int C, int Hs, int Ws, int H, int W, int k_rt, int accumulate, int nhwc, int do_gs) {
+                 int B, int C, int Hs, int Ws, int H, int W, int k_rt, int accumulate, int nhwc) {
     using A = typename Acc<T>::type;
     const int k = K ? K : k_rt, KK = k * k;
     const long long hw = (long long)H * W, total = (long long)B * hw;
@@ -189,15 +153,9 @@ k_local_attn_bwd(const T* __restrict__ src, const TF* __restrict__ flow, const T
     A gfx = static_cast<A>(0), gfy = static_cast<A>(0);
 
     bool regular = false;
-    if (K > 0) {
-        AxisTap<A> tx[K ? K : 1], ty[K ? K : 1];
-        regular = true;
-#pragma unroll
-        for (int j = 0; j < K; ++j) {
-            tx[j] = axis_tap<A>(flow_x, j - K / 2, x, Ws);
-            ty[j] = axis_tap<A>(flow_y, j - K / 2, y, Hs);
-            regular = regular && (tx[j].fl == tx[0].fl + j) && (ty[j].fl == ty[0].fl + j);
-        }
+    if constexpr (K > 0) {
+        AxisTap<A> tx[K], ty[K];
+        regular = taps_regular<A, K>(flow_x, flow_y, x, y, Hs, Ws, tx, ty);
         if (regular) {
             constexpr int K1 = K + 1;
             A Wc[K1 * K1], Q[K1 * K1];
@@ -227,20 +185,15 @@ k_local_attn_bwd(const T* __restrict__ src, const TF* __restrict__ flow, const T
                     for (int q = 0; q < K1; ++q) {
                         const int o = cy[r] + cx[q];
                         Q[r * K1 + q] += g * ld(s + o);
-                        if (do_gs) red_add(gs + o, g * Wc[r * K1 + q]);
+                        red_add(gs + o, g * Wc[r * K1 + q]);
                     }
             }
 #pragma unroll
             for (int i = 0; i < K; ++i)
 #pragma unroll
-                for (int j = 0; j < K; ++j) {
-                    const A qLT = Q[i * K1 + j], qRT = Q[i * K1 + j + 1], qLB = Q[(i + 1) * K1 + j], qRB = Q[(i + 1) * K1 + j + 1];
-                    dp[i * K + j] = inv_kk * (ty[i].wlo * (tx[j].wlo * qLT + tx[j].whi * qRT) +
-                                              ty[i].whi * (tx[j].wlo * qLB + tx[j].whi * qRB));
-                    const A pij = p[i * K + j] * inv_kk;
-                    gfy += pij * (-tx[j].wlo * qLT - tx[j].whi * qRT + tx[j].wlo * qLB + tx[j].whi * qRB);
-                    gfx += pij * (-ty[i].wlo * qLT - ty[i].whi * qLB + ty[i].wlo * qRT + ty[i].whi * qRB);
-                }
+                for (int j = 0; j < K; ++j)
+                    dp[i * K + j] = tap_backward<A>(tx[j], ty[i], p[i * K + j] * inv_kk, inv_kk, Q[i * K1 + j], Q[i * K1 + j + 1],
+                                                    Q[(i + 1) * K1 + j], Q[(i + 1) * K1 + j + 1], gfx, gfy);
         }
     }
     if (!regular) {
@@ -255,36 +208,22 @@ k_local_attn_bwd(const T* __restrict__ src, const TF* __restrict__ flow, const T
                 const T* sq = s;
                 T* gc = gs;
                 const T* goc = go;
+#pragma unroll 1   // rare path, k*k copies of this loop: unrolled, it would raise the register pressure of the whole kernel
                 for (int c = 0; c < C; ++c, sq += sc, gc += sc, goc += oc) {
                     const A g = ld(goc);
                     qLT += g * ld(sq + oLT); qRT += g * ld(sq + oRT); qLB += g * ld(sq + oLB); qRB += g * ld(sq + oRB);
                     const A gp = g * pij;
-                    if (do_gs) {
-                        red_add(gc + oLT, gp * (tx.wlo * ty.wlo));
-                        red_add(gc + oRT, gp * (tx.whi * ty.wlo));
-                        red_add(gc + oLB, gp * (tx.wlo * ty.whi));
-                        red_add(gc + oRB, gp * (tx.whi * ty.whi));
-                    }
+                    red_add(gc + oLT, gp * (tx.wlo * ty.wlo));
+                    red_add(gc + oRT, gp * (tx.whi * ty.wlo));
+                    red_add(gc + oLB, gp * (tx.wlo * ty.whi));
+                    red_add(gc + oRB, gp * (tx.whi * ty.whi));
                 }
-                dp[i * k + j] = inv_kk * (ty.wlo * (tx.wlo * qLT + tx.whi * qRT) + ty.whi * (tx.wlo * qLB + tx.whi * qRB));
-                gfy += pij * (-tx.wlo * qLT - tx.whi * qRT + tx.wlo * qLB + tx.whi * qRB);
-                gfx += pij * (-ty.wlo * qLT - ty.whi * qLB + ty.wlo * qRT + ty.whi * qRB);
+                dp[i * k + j] = tap_backward<A>(tx, ty, pij, inv_kk, qLT, qRT, qLB, qRB, gfx, gfy);
             }
         }
     }
-    // softmax backward: dl_t = p_t * (dp_t - sum_u p_u dp_u)
-    A dot = static_cast<A>(0);
-#pragma unroll
-    for (int t = 0; t < (K ? K * K : KK); ++t) dot += p[t] * dp[t];
-    T* gl = glogits + (long long)b * KK * hw + pofs;
-#pragma unroll
-    for (int t = 0; t < (K ? K * K : KK); ++t) {
-        const A v = p[t] * (dp[t] - dot);
-        st(gl + t * hw, accumulate ? static_cast<A>(ld(gl + t * hw)) + v : v);
-    }
-    TF* gf = gflow + (long long)b * 2 * hw + pofs;
-    st(gf, accumulate ? static_cast<A>(ld(gf)) + gfx : gfx);
-    st(gf + hw, accumulate ? static_cast<A>(ld(gf + hw)) + gfy : gfy);
+    store_pixel_grads<T, TF, A, K * K>(p, dp, KK, gfx, gfy, glogits + (long long)b * KK * hw + pofs,
+                                       gflow + (long long)b * 2 * hw + pofs, hw, accumulate);
 }
 
 template <typename T, typename TF, int K>
@@ -301,12 +240,12 @@ static int la_launch_fwd(const void* src, const void* flow, const void* logits, 
 template <typename T, typename TF, int K>
 static int la_launch_bwd(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc,
                          void* gflow, void* glogits, int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate,
-                         int nhwc, int do_gs, cudaStream_t st_) {
+                         int nhwc, cudaStream_t st_) {
     const long long total = (long long)B * H * W;
     const int threads = 128;
     k_local_attn_bwd<T, TF, K><<<(unsigned)((total + threads - 1) / threads), threads, 0, st_>>>(
         (const T*)src, (const TF*)flow, (const T*)logits, (const T*)gout, (T*)gsrc, (TF*)gflow, (T*)glogits, B, C, Hs,
-        Ws, H, W, k, accumulate, nhwc, do_gs);
+        Ws, H, W, k, accumulate, nhwc);
     return launch_status();
 }
 
@@ -319,41 +258,29 @@ static int la_launch_bwd(const void* src, const void* flow, const void* logits, 
         default: return fn<T, TF, 0>(__VA_ARGS__);     \
     }
 
-template <typename T, typename TF>
-static int la_fwd_k(const void* src, const void* flow, const void* logits, void* out, void* probs, const void* prev,
-                    const void* mask, int B, int C, int Hs, int Ws, int H, int W, int k, int nhwc, cudaStream_t st_) {
-    GFLA_K_DISPATCH(la_launch_fwd, src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, k, nhwc, st_)
-}
-template <typename T, typename TF>
-static int la_bwd_k(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow,
-                    void* glogits, int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate, int nhwc, int do_gs,
-                    cudaStream_t st_) {
-    GFLA_K_DISPATCH(la_launch_bwd, src, flow, logits, gout, gsrc, gflow, glogits, B, C, Hs, Ws, H, W, k, accumulate, nhwc, do_gs, st_)
-}
-
 int local_attn_fwd_gather(const void* src, const void* flow, const void* logits, void* out, void* probs, const void* prev,
                           const void* mask, int B, int C, int Hs, int Ws, int H, int W, int k, int dtype, int flow_dtype,
                           int layout, cudaStream_t st_) {
     const int nhwc = layout == GFLA_NHWC;
-    return GFLA_DISPATCH_T(dtype, [&]() -> int {
-        if (flow_dtype == dtype) return la_fwd_k<T, T>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, k, nhwc, st_);
-        return la_fwd_k<T, float>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, k, nhwc, st_);
+    return dispatch_dtypes(dtype, flow_dtype, dtype, [&](auto t, auto tf, auto) -> int {
+        using T = typename decltype(t)::type;
+        using TF = typename decltype(tf)::type;
+        GFLA_K_DISPATCH(la_launch_fwd, src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, k, nhwc, st_)
     });
 }
 
 int local_attn_bwd_gather(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc,
                           void* gflow, void* glogits, int B, int C, int Hs, int Ws, int H, int W, int k, int dtype,
-                          int flow_dtype, int accumulate, int layout, int do_gs, cudaStream_t st_) {
-    // do_gs = 0: grad_source is produced elsewhere (tile kernel); only grad_flow / grad_logits here
+                          int flow_dtype, int accumulate, int layout, cudaStream_t st_) {
     const int nhwc = layout == GFLA_NHWC;
-    if (!accumulate && do_gs) {
+    if (!accumulate) {
         const int e = zero_async(gsrc, (size_t)B * C * Hs * Ws * elem_size(dtype), st_);
         if (e != GFLA_OK) return e;
     }
-    return GFLA_DISPATCH_T(dtype, [&]() -> int {
-        if (flow_dtype == dtype)
-            return la_bwd_k<T, T>(src, flow, logits, gout, gsrc, gflow, glogits, B, C, Hs, Ws, H, W, k, accumulate, nhwc, do_gs, st_);
-        return la_bwd_k<T, float>(src, flow, logits, gout, gsrc, gflow, glogits, B, C, Hs, Ws, H, W, k, accumulate, nhwc, do_gs, st_);
+    return dispatch_dtypes(dtype, flow_dtype, dtype, [&](auto t, auto tf, auto) -> int {
+        using T = typename decltype(t)::type;
+        using TF = typename decltype(tf)::type;
+        GFLA_K_DISPATCH(la_launch_bwd, src, flow, logits, gout, gsrc, gflow, glogits, B, C, Hs, Ws, H, W, k, accumulate, nhwc, st_)
     });
 }
 

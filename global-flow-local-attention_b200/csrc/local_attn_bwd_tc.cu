@@ -4,7 +4,8 @@
 // Per 16x8 pixel group and 16-position row segment of the group's tap footprint (channels in passes of CN):
 //   * P[128 px][16 pos] = G[128 px][CN] * S[16 pos][CN]^T    the grad_out . source dot products of every pixel with
 //     every position of the segment; each pixel thread then picks its (k+1)^2 window entries out of P into Q (registers).
-//     Q is exactly the CUDA-core kernel's Q (local_attn.cu), so grad_flow / grad_logits follow from it per pixel;
+//     Q is exactly the CUDA-core kernel's Q (local_attn.cu), so grad_flow / grad_logits follow from it per pixel with
+//     the same formulas (local_attn_pixel.cuh);
 //   * GS[16 pos][CN] = Wfull^T[16 pos][128 px] * G[128 px][CN] grad_source of the segment, added with bf16x2 atomics
 //     (the caller's buffer is zero-filled first unless the call accumulates).
 // The grad_out tile G stays in shared memory for the whole pass; the source segment arrives by cp.async one step ahead.
@@ -40,7 +41,7 @@ __device__ __forceinline__ void irregular_pixel_bwd(const __nv_bfloat16* __restr
     const long long hw = (long long)H * W, qofs = (long long)qy * W + qx;
     const float fx = flow[(long long)b * 2 * hw + qofs], fy = flow[(long long)b * 2 * hw + hw + qofs];
     float p[KK], dp[KK];
-    pixel_softmax_f32<KK>(logits + (long long)b * KK * hw + qofs, hw, p);
+    pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + qofs, hw, KK, p);
     const float inv_kk = 1.0f / static_cast<float>(KK);
     const __nv_bfloat16* s = src + (long long)b * Hs * Ws * C;
     __nv_bfloat16* gs = gsrc + (long long)b * Hs * Ws * C;
@@ -72,24 +73,12 @@ __device__ __forceinline__ void irregular_pixel_bwd(const __nv_bfloat16* __restr
             for (int t = 0; t < 4; ++t)
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) q[t] += __shfl_xor_sync(0xffffffffu, q[t], o);
-            dp[i * K + j] = inv_kk * (ty.wlo * (tx.wlo * q[0] + tx.whi * q[1]) + ty.whi * (tx.wlo * q[2] + tx.whi * q[3]));
-            gfy += pij * (-tx.wlo * q[0] - tx.whi * q[1] + tx.wlo * q[2] + tx.whi * q[3]);
-            gfx += pij * (-ty.wlo * q[0] - ty.whi * q[2] + ty.wlo * q[1] + ty.whi * q[3]);
+            dp[i * K + j] = tap_backward<float>(tx, ty, pij, inv_kk, q[0], q[1], q[2], q[3], gfx, gfy);
         }
     }
-    if (lane != 0) return;
-    float dot = 0.f;
-#pragma unroll
-    for (int t = 0; t < KK; ++t) dot += p[t] * dp[t];
-    __nv_bfloat16* gl = glogits + (long long)b * KK * hw + qofs;
-#pragma unroll
-    for (int t = 0; t < KK; ++t) {
-        const float v = p[t] * (dp[t] - dot);
-        gl[t * hw] = __float2bfloat16_rn(accumulate ? __bfloat162float(gl[t * hw]) + v : v);
-    }
-    float* gf = gflow + (long long)b * 2 * hw + qofs;
-    gf[0] = accumulate ? gf[0] + gfx : gfx;
-    gf[hw] = accumulate ? gf[hw] + gfy : gfy;
+    if (lane == 0)
+        store_pixel_grads<__nv_bfloat16, float, float, KK>(p, dp, KK, gfx, gfy, glogits + (long long)b * KK * hw + qofs,
+                                                           gflow + (long long)b * 2 * hw + qofs, hw, accumulate);
 }
 
 template <int K, int CN>
@@ -104,13 +93,9 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     int* irr = reinterpret_cast<int*>(smem + L::IRR);
     int& nirr = irr[128];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
-    FastDiv fc, fr;
-    fc.init(gcols);
-    fr.init(grows);
-    uint32_t g = blockIdx.x, gc, gr, b;
-    fc.divmod(g, g, gc);
-    fr.divmod(g, b, gr);
-    const int gx0 = gc * GW, gy0 = gr * GH;
+    uint32_t b;
+    int gx0, gy0;
+    group_decode(gcols, grows, b, gx0, gy0);
     const long long hw = (long long)H * W;
     const float inv_kk = 1.0f / static_cast<float>(KK);
 
@@ -127,9 +112,9 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     bool regular = false;
     if (valid) {
         float p[KK];
-        pixel_softmax_f32<KK>(logits + (long long)b * KK * hw + pofs, hw, p);
+        pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
         AxisTap<float> tx[K], ty[K];
-        regular = taps_regular<K>(flow[(long long)b * 2 * hw + pofs], flow[(long long)b * 2 * hw + hw + pofs], px, py, Hs, Ws, tx, ty);
+        regular = taps_regular<float, K>(flow[(long long)b * 2 * hw + pofs], flow[(long long)b * 2 * hw + hw + pofs], px, py, Hs, Ws, tx, ty);
         if (regular) {
             X0u = tx[0].fl;
             Y0u = ty[0].fl;
@@ -139,7 +124,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
         }
     }
     int bx0, by0, bx1, by1;
-    group_bbox<K>(flow, b, gx0, gy0, H, W, Hs, Ws, lane, false, bx0, by0, bx1, by1);
+    group_bbox<K>(flow, b, gx0, gy0, H, W, Hs, Ws, lane, bx0, by0, bx1, by1);
     const int nseg = (bx1 - bx0) / SEG + 1, nsteps = nseg * (by1 - by0 + 1);
 
     const uint32_t sb = smem_u32(smem);
@@ -177,25 +162,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
             const int y = by0 + s / nseg, x = bx0 + (s % nseg) * SEG;
             const uint32_t aw = aw_base + buf * (SEG * BT_AWSTR);
             // this pixel's column of Wfull^T for the segment (slab zeroed one step earlier); zero the other slab's share
-            if (regular) {
-                const int rr = y - Y0;
-                if (rr >= 0 && rr <= K) {
-                    float wr[K1];
-#pragma unroll
-                    for (int t = 0; t < K1; ++t) wr[t] = 0.f;
-#pragma unroll
-                    for (int r = 0; r < K1; ++r)
-                        if (rr == r) {
-#pragma unroll
-                            for (int t = 0; t < K1; ++t) wr[t] = w[r * K1 + t];
-                        }
-#pragma unroll
-                    for (int t = 0; t < K1; ++t) {
-                        const int e = X0 + t - x;
-                        if (e >= 0 && e < SEG && wr[t] != 0.f) sts16(aw + e * BT_AWSTR + tid * 2, bf16_bits(wr[t]));
-                    }
-                }
-            }
+            if (regular) scatter_window_row<K>(aw + tid * 2, BT_AWSTR, w, X0, Y0, y, x);
             {
                 const uint32_t z = aw_base + (buf ^ 1) * (SEG * BT_AWSTR) + (tid >> 3) * BT_AWSTR + (tid & 7) * 32;
                 sts128(z, 0u, 0u, 0u, 0u);
@@ -286,35 +253,21 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
         }
     }
 
-    // ---- regular pixels: grad_logits and grad_flow from Q (the formulas of local_attn.cu)
+    // ---- regular pixels: grad_logits and grad_flow from Q (local_attn_pixel.cuh)
     if (regular) {
         float p[KK], dp[KK];
-        pixel_softmax_f32<KK>(logits + (long long)b * KK * hw + pofs, hw, p);
+        pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
         AxisTap<float> tx[K], ty[K];
-        taps_regular<K>(flow[(long long)b * 2 * hw + pofs], flow[(long long)b * 2 * hw + hw + pofs], px, py, Hs, Ws, tx, ty);
+        taps_regular<float, K>(flow[(long long)b * 2 * hw + pofs], flow[(long long)b * 2 * hw + hw + pofs], px, py, Hs, Ws, tx, ty);
         float gfx = 0.f, gfy = 0.f;
 #pragma unroll
         for (int i = 0; i < K; ++i)
 #pragma unroll
-            for (int j = 0; j < K; ++j) {
-                const float qLT = Q[i * K1 + j], qRT = Q[i * K1 + j + 1], qLB = Q[(i + 1) * K1 + j], qRB = Q[(i + 1) * K1 + j + 1];
-                dp[i * K + j] = inv_kk * (ty[i].wlo * (tx[j].wlo * qLT + tx[j].whi * qRT) + ty[i].whi * (tx[j].wlo * qLB + tx[j].whi * qRB));
-                const float pij = p[i * K + j] * inv_kk;
-                gfy += pij * (-tx[j].wlo * qLT - tx[j].whi * qRT + tx[j].wlo * qLB + tx[j].whi * qRB);
-                gfx += pij * (-ty[i].wlo * qLT - ty[i].whi * qLB + ty[i].wlo * qRT + ty[i].whi * qRB);
-            }
-        float dot = 0.f;
-#pragma unroll
-        for (int t = 0; t < KK; ++t) dot += p[t] * dp[t];
-        __nv_bfloat16* gl = glogits + (long long)b * KK * hw + pofs;
-#pragma unroll
-        for (int t = 0; t < KK; ++t) {
-            const float v = p[t] * (dp[t] - dot);
-            gl[t * hw] = __float2bfloat16_rn(accumulate ? __bfloat162float(gl[t * hw]) + v : v);
-        }
-        float* gf = gflow + (long long)b * 2 * hw + pofs;
-        gf[0] = accumulate ? gf[0] + gfx : gfx;
-        gf[hw] = accumulate ? gf[hw] + gfy : gfy;
+            for (int j = 0; j < K; ++j)
+                dp[i * K + j] = tap_backward<float>(tx[j], ty[i], p[i * K + j] * inv_kk, inv_kk, Q[i * K1 + j], Q[i * K1 + j + 1],
+                                                    Q[(i + 1) * K1 + j], Q[(i + 1) * K1 + j + 1], gfx, gfy);
+        store_pixel_grads<__nv_bfloat16, float, float, KK>(p, dp, KK, gfx, gfy, glogits + (long long)b * KK * hw + pofs,
+                                                           gflow + (long long)b * 2 * hw + pofs, hw, accumulate);
     }
     // ---- pixels with non-consecutive taps: literal arithmetic, one warp per pixel
     for (int i = warp; i < nirr; i += BT_THREADS / 32) {

@@ -60,30 +60,6 @@ __device__ __forceinline__ void seg_store(uint32_t dst, int tid, const SegLoad<N
     }
 }
 
-// this pixel's row of the weight slab for source row y, positions [x, x + 16): zeros except the window row y - Y0
-template <int K>
-__device__ __forceinline__ void slab_row(uint32_t row, bool regular, const float* w, int X0, int Y0, int y, int x) {
-    constexpr int K1 = K + 1;
-    sts128(row, 0u, 0u, 0u, 0u);
-    sts128(row + 16, 0u, 0u, 0u, 0u);
-    const int rr = y - Y0;
-    if (!regular || rr < 0 || rr > K) return;
-    float wr[K1];
-#pragma unroll
-    for (int s = 0; s < K1; ++s) wr[s] = 0.f;
-#pragma unroll
-    for (int r = 0; r < K1; ++r)
-        if (rr == r) {
-#pragma unroll
-            for (int s = 0; s < K1; ++s) wr[s] = w[r * K1 + s];
-        }
-#pragma unroll
-    for (int s = 0; s < K1; ++s) {
-        const int e = X0 + s - x;
-        if (e >= 0 && e < SEG && wr[s] != 0.f) sts16(row + e * 2, bf16_bits(wr[s]));
-    }
-}
-
 template <int K, bool NHWC>
 __global__ void __launch_bounds__(FT_THREADS, 1)
 k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow, const __nv_bfloat16* __restrict__ logits,
@@ -92,13 +68,9 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     constexpr int K1 = K + 1, KK = K * K;
     __shared__ FwdSmem sm;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
-    FastDiv fc, fr;
-    fc.init(gcols);
-    fr.init(grows);
-    uint32_t g = blockIdx.x, gc, gr, b;
-    fc.divmod(g, g, gc);
-    fr.divmod(g, b, gr);
-    const int gx0 = gc * GW, gy0 = gr * GH;
+    uint32_t b;
+    int gx0, gy0;
+    group_decode(gcols, grows, b, gx0, gy0);
     const long long hw = (long long)H * W;
 
     if (tid == 0) sm.nirr = 0;
@@ -112,18 +84,18 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     if (valid) {
         const long long pofs = (long long)py * W + px;
         float p[KK];
-        pixel_softmax_f32<KK>(logits + (long long)b * KK * hw + pofs, hw, p);
+        pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
         if (probs != nullptr) {
 #pragma unroll
             for (int t = 0; t < KK; ++t) probs[(long long)b * KK * hw + t * hw + pofs] = __float2bfloat16_rn(p[t]);
         }
         AxisTap<float> tx[K], ty[K];
-        regular = taps_regular<K>(flow[(long long)b * 2 * hw + pofs], flow[(long long)b * 2 * hw + hw + pofs], px, py, Hs, Ws, tx, ty);
+        regular = taps_regular<float, K>(flow[(long long)b * 2 * hw + pofs], flow[(long long)b * 2 * hw + hw + pofs], px, py, Hs, Ws, tx, ty);
         if (regular) build_window<K>(p, tx, ty, Hs, Ws, 1.0f / static_cast<float>(KK), w, X0, Y0);
         else sm.irr[atomicAdd(&sm.nirr, 1)] = tid;
     }
     int bx0, by0, bx1, by1;
-    group_bbox<K>(flow, b, gx0, gy0, H, W, Hs, Ws, lane, false, bx0, by0, bx1, by1);
+    group_bbox<K>(flow, b, gx0, gy0, H, W, Hs, Ws, lane, bx0, by0, bx1, by1);
     const int nseg = (bx1 - bx0) / SEG + 1, nsteps = nseg * (by1 - by0 + 1);
 
     const uint32_t a_base = smem_u32(sm.a[0]), b_base = smem_u32(sm.b[0]);
@@ -147,7 +119,11 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
         for (int s = 0; s < nsteps; ++s) {
             const int buf = s & 1;
             const int y = by0 + s / nseg, x = bx0 + (s % nseg) * SEG;
-            slab_row<K>(a_row + buf * (128 * FT_ASTR), regular, w, X0, Y0, y, x);
+            // this pixel's row of the weight slab: zeros except window row y - Y0
+            const uint32_t row = a_row + buf * (128 * FT_ASTR);
+            sts128(row, 0u, 0u, 0u, 0u);
+            sts128(row + 16, 0u, 0u, 0u, 0u);
+            if (regular) scatter_window_row<K>(row, 2, w, X0, Y0, y, x);
             if (NHWC) cp_async_wait_all();
             __syncthreads();      // slab and segment of step s complete; everybody is past step s-1's MMAs
             const bool more = s + 1 < nsteps;
@@ -206,7 +182,7 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     for (int i = warp; i < sm.nirr; i += FT_THREADS / 32) {
         const int m = sm.irr[i], qx = gx0 + (m & 15), qy = gy0 + (m >> 4);
         const long long qofs = (long long)qy * W + qx;
-        irregular_pixel<K, NHWC>(src, logits, out, prev, mask, b, C, 0, C, Hs, Ws, H, W, qx, qy, flow[(long long)b * 2 * hw + qofs],
+        irregular_pixel<K, NHWC>(src, logits, out, prev, mask, b, C, Hs, Ws, H, W, qx, qy, flow[(long long)b * 2 * hw + qofs],
                                  flow[(long long)b * 2 * hw + hw + qofs], lane);
     }
 }
@@ -225,9 +201,7 @@ static int launch_fwd(const void* src, const void* flow, const void* logits, voi
 
 }  // namespace tc
 
-bool local_attn_fwd_tc_supported(int B, int C, int Hs, int Ws, int H, int W, int k, int dtype, int flow_dtype,
-                                 int layout, const void* src, const void* out) {
-    (void)B; (void)H; (void)W; (void)Hs;
+bool local_attn_fwd_tc_supported(int C, int Ws, int k, int dtype, int flow_dtype, int layout, const void* src, const void* out) {
     const bool c_ok = C % 256 == 0 || C == 128 || C == 64;
     if (!(dtype == GFLA_BF16 && flow_dtype == GFLA_F32 && (k == 3 || k == 5) && c_ok && aligned(src, 16))) return false;
     // channels-last: 16-byte cp.async of the source and 4-byte channel-pair stores need aligned pointers
@@ -237,7 +211,7 @@ bool local_attn_fwd_tc_supported(int B, int C, int Hs, int Ws, int H, int W, int
 int local_attn_fwd_tc(const void* src, const void* flow, const void* logits, void* out, void* probs, const void* prev,
                       const void* mask, int B, int C, int Hs, int Ws, int H, int W, int k, int dtype, int flow_dtype,
                       int layout, cudaStream_t st_) {
-    if (!local_attn_fwd_tc_supported(B, C, Hs, Ws, H, W, k, dtype, flow_dtype, layout, src, out)) return GFLA_E_NOTSUP;
+    if (!local_attn_fwd_tc_supported(C, Ws, k, dtype, flow_dtype, layout, src, out)) return GFLA_E_NOTSUP;
     const bool nhwc = layout == GFLA_NHWC;
     if (k == 5) return nhwc ? tc::launch_fwd<5, true>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, st_)
                             : tc::launch_fwd<5, false>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, st_);

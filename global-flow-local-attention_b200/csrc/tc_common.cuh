@@ -16,7 +16,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast
 __device__ __forceinline__ void sts128(uint32_t a, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
 }
-__device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 __device__ __forceinline__ void sts16(uint32_t a, uint32_t v) {
     asm volatile("{\n\t.reg .b16 h;\n\tcvt.u16.u32 h, %1;\n\tst.shared.b16 [%0], h;\n\t}" ::"r"(a), "r"(v) : "memory");
 }
