@@ -10,6 +10,8 @@
 //     (the caller's buffer is zero-filled first unless the call accumulates).
 // The grad_out tile G stays in shared memory for the whole pass; the source segment arrives by cp.async one step ahead.
 // Warp w owns pixel rows 32w..32w+31 of the P GEMM and channels [w CN/4, (w+1) CN/4) of the GS GEMM (mma.sync m16n8k16).
+// A 16-pixel group row none of whose windows meets the step (window_meets_step) is skipped as a P m-tile and as a GS
+// k-step; the warps publish these row bits next to the step's weight slab.  Steps that no pixel touches do no MMAs.
 // Pixels whose taps are not consecutive integers take the reference's literal 4-tap arithmetic, one warp per pixel.
 #include "tile_window.cuh"
 
@@ -28,8 +30,30 @@ struct BwdSmem {
     static constexpr int AW = S + 2 * SEG * GSTR;
     static constexpr int P = AW + 2 * SEG * BT_AWSTR;
     static constexpr int IRR = P + 128 * BT_PSTR * 4;
-    static constexpr int ALLOC = IRR + 129 * 4;
+    static constexpr int ROWS = IRR + 129 * 4;      // per slab buffer: byte w = warp_row_bits of warp w for the step
+    static constexpr int ALLOC = ROWS + 2 * 4;
 };
+
+// P GEMM of one warp for one step: the m-tiles whose pixel row is active (M0, M1) of its 32 pixels x 16 positions
+template <int CN, bool M0, bool M1>
+__device__ __forceinline__ void p_gemm(uint32_t ga, uint32_t sf, float (&pacc)[2][2][4]) {
+    constexpr int GSTR = BwdSmem<CN>::GSTR;
+#pragma unroll 4
+    for (int kk = 0; kk < CN / 16; ++kk) {
+        uint32_t a0[4], a1[4], bf[4];
+        if (M0) ldsm_x4(ga + kk * 32, a0);
+        if (M1) ldsm_x4(ga + 16 * GSTR + kk * 32, a1);
+        ldsm_x4(sf + kk * 32, bf);
+        if (M0) {
+            mma_bf16(pacc[0][0], a0, bf[0], bf[1]);
+            mma_bf16(pacc[0][1], a0, bf[2], bf[3]);
+        }
+        if (M1) {
+            mma_bf16(pacc[1][0], a1, bf[0], bf[1]);
+            mma_bf16(pacc[1][1], a1, bf[2], bf[3]);
+        }
+    }
+}
 
 template <int K>
 __device__ __forceinline__ void irregular_pixel_bwd(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow,
@@ -92,6 +116,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     extern __shared__ __align__(16) unsigned char smem[];
     int* irr = reinterpret_cast<int*>(smem + L::IRR);
     int& nirr = irr[128];
+    unsigned char* rows = smem + L::ROWS;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
     uint32_t b;
     int gx0, gy0;
@@ -105,7 +130,8 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     const int px = gx0 + (tid & 15), py = gy0 + (tid >> 4);
     const bool valid = px < W && py < H;
     const long long pofs = (long long)py * W + px;
-    float w[K1 * K1], Q[K1 * K1];
+    uint32_t w[K1 * K1 / 2];
+    float Q[K1 * K1];
 #pragma unroll
     for (int i = 0; i < K1 * K1; ++i) Q[i] = 0.f;
     int X0 = 0, Y0 = 0, X0u = 0, Y0u = 0;
@@ -125,7 +151,6 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     }
     int bx0, by0, bx1, by1;
     group_bbox<K>(flow, b, gx0, gy0, H, W, Hs, Ws, lane, bx0, by0, bx1, by1);
-    const int nseg = (bx1 - bx0) / SEG + 1, nsteps = nseg * (by1 - by0 + 1);
 
     const uint32_t sb = smem_u32(smem);
     const uint32_t g_base = sb + L::G, s_base = sb + L::S, aw_base = sb + L::AW, p_base = sb + L::P;
@@ -140,8 +165,10 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
 
     for (int c0 = 0; c0 < C; c0 += CN) {
         __syncthreads();          // the previous pass is done with G, S and the weight slabs
-        // grad_out tile of the group (pixels outside the image: zeros), then the first source segment
-#pragma unroll
+        // grad_out tile of the group (pixels outside the image: zeros), then the first source segment.  Not fully
+        // unrolled: the compiler would then keep all CN/8 pass-invariant 64-bit addresses live across the step loop, and
+        // at CN = 256 that spills.
+#pragma unroll 4
         for (int i = 0; i < CN / 8; ++i) {
             const int idx = i * BT_THREADS + tid, m = idx / (CN / 8), j = idx % (CN / 8);
             const int qx = gx0 + (m & 15), qy = gy0 + (m >> 4);
@@ -157,99 +184,106 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
         sts128(aw_base + (tid >> 3) * BT_AWSTR + (tid & 7) * 32, 0u, 0u, 0u, 0u);
         sts128(aw_base + (tid >> 3) * BT_AWSTR + (tid & 7) * 32 + 16, 0u, 0u, 0u, 0u);
         __syncthreads();          // slab 0 zeroed before anybody scatters into it
-        for (int s = 0; s < nsteps; ++s) {
+        // steps walk the footprint row-major: y from by0, x = bx0, bx0 + SEG, ... while x <= bx1
+        for (int s = 0, y = by0, x = bx0; y <= by1; ++s) {
             const int buf = s & 1;
-            const int y = by0 + s / nseg, x = bx0 + (s % nseg) * SEG;
+            int xn = x + SEG, yn = y;
+            if (xn > bx1) { xn = bx0; ++yn; }
             const uint32_t aw = aw_base + buf * (SEG * BT_AWSTR);
             // this pixel's column of Wfull^T for the segment (slab zeroed one step earlier); zero the other slab's share
-            if (regular) scatter_window_row<K>(aw + tid * 2, BT_AWSTR, w, X0, Y0, y, x);
+            const bool act = regular && window_meets_step<K>(X0u, Y0u, Hs, Ws, y, x);
+            if (act) scatter_window_row<K>(aw + tid * 2, BT_AWSTR, w, X0, Y0, y, x);
             {
+                const uint32_t rb = warp_row_bits(act);
+                if (lane == 0) rows[buf * 4 + warp] = static_cast<unsigned char>(rb);
                 const uint32_t z = aw_base + (buf ^ 1) * (SEG * BT_AWSTR) + (tid >> 3) * BT_AWSTR + (tid & 7) * 32;
                 sts128(z, 0u, 0u, 0u, 0u);
                 sts128(z + 16, 0u, 0u, 0u, 0u);
             }
             cp_async_wait_all();
-            __syncthreads();      // G, segment s and slab s complete; everybody is past step s-1
-            if (s + 1 < nsteps) {
-                const int yn = by0 + (s + 1) / nseg, xn = bx0 + ((s + 1) % nseg) * SEG, i = tid >> 3;
+            __syncthreads();      // G, segment s, slab s and its row bits complete; everybody is past step s-1
+            if (yn <= by1) {
+                const int i = tid >> 3;
                 const uint32_t dst = s_base + (buf ^ 1) * (SEG * GSTR) + i * GSTR;
                 const __nv_bfloat16* sp = s_b + ((long long)yn * Ws + min(xn + i, Ws - 1)) * C + c0;
                 for (int j = tid & 7; j < CN / 8; j += 8) cp_async16(dst + j * 16, sp + j * 8);
                 cp_async_commit();
             }
-            // P = G * S^T: this warp's 32 pixels x 16 positions
-            float pacc[2][2][4];
+            // group rows with an active pixel: bit 8 v + h = group row 2 v + h (the same word in every thread)
+            const uint32_t grows_on = *reinterpret_cast<const uint32_t*>(rows + buf * 4);
+            if (grows_on != 0u) {
+                // P = G * S^T: this warp's 32 pixels x 16 positions, m-tiles of inactive pixel rows skipped
+                float pacc[2][2][4];
 #pragma unroll
-            for (int mt = 0; mt < 2; ++mt)
+                for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-                for (int nt = 0; nt < 2; ++nt)
+                    for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) pacc[mt][nt][q] = 0.f;
-            const uint32_t sf = s_frag_b + buf * (SEG * GSTR);
-#pragma unroll 4
-            for (int kk = 0; kk < CN / 16; ++kk) {
-                uint32_t a0[4], a1[4], bf[4];
-                ldsm_x4(g_frag_a + kk * 32, a0);
-                ldsm_x4(g_frag_a + 16 * GSTR + kk * 32, a1);
-                ldsm_x4(sf + kk * 32, bf);
-                mma_bf16(pacc[0][0], a0, bf[0], bf[1]);
-                mma_bf16(pacc[0][1], a0, bf[2], bf[3]);
-                mma_bf16(pacc[1][0], a1, bf[0], bf[1]);
-                mma_bf16(pacc[1][1], a1, bf[2], bf[3]);
-            }
-            // GS = Wfull^T * G: 16 positions x this warp's CN/4 channels
-            float gacc[NTW][4];
+                        for (int q = 0; q < 4; ++q) pacc[mt][nt][q] = 0.f;
+                const uint32_t sf = s_frag_b + buf * (SEG * GSTR);
+                const uint32_t pm = (grows_on >> (8 * warp)) & 3u;
+                if (pm == 3u) p_gemm<CN, true, true>(g_frag_a, sf, pacc);
+                else if (pm == 1u) p_gemm<CN, true, false>(g_frag_a, sf, pacc);
+                else if (pm == 2u) p_gemm<CN, false, true>(g_frag_a, sf, pacc);
+                // GS = Wfull^T * G: 16 positions x this warp's CN/4 channels; the k-steps of inactive pixel rows add zeros
+                float gacc[NTW][4];
 #pragma unroll
-            for (int nt = 0; nt < NTW; ++nt)
+                for (int nt = 0; nt < NTW; ++nt)
 #pragma unroll
-                for (int q = 0; q < 4; ++q) gacc[nt][q] = 0.f;
+                    for (int q = 0; q < 4; ++q) gacc[nt][q] = 0.f;
 #pragma unroll
-            for (int kk = 0; kk < 128 / 16; ++kk) {
-                uint32_t af[4];
-                ldsm_x4(aw_frag + buf * (SEG * BT_AWSTR) + kk * 32, af);
+                for (int kk = 0; kk < 128 / 16; ++kk) {
+                    if (((grows_on >> (8 * (kk >> 1) + (kk & 1))) & 1u) == 0u) continue;
+                    uint32_t af[4];
+                    ldsm_x4(aw_frag + buf * (SEG * BT_AWSTR) + kk * 32, af);
 #pragma unroll
-                for (int np = 0; np < NTW / 2; ++np) {
-                    uint32_t bg[4];
-                    ldsm_x4_t(g_frag_b + kk * 16 * GSTR + np * 32, bg);
-                    mma_bf16(gacc[2 * np], af, bg[0], bg[1]);
-                    mma_bf16(gacc[2 * np + 1], af, bg[2], bg[3]);
+                    for (int np = 0; np < NTW / 2; ++np) {
+                        uint32_t bg[4];
+                        ldsm_x4_t(g_frag_b + kk * 16 * GSTR + np * 32, bg);
+                        mma_bf16(gacc[2 * np], af, bg[0], bg[1]);
+                        mma_bf16(gacc[2 * np + 1], af, bg[2], bg[3]);
+                    }
                 }
-            }
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int xp = x + gid + 8 * h;
-                if (xp > bx1) continue;
-                __nv_bfloat16* d = gs_b + ((long long)y * Ws + xp) * C + c0 + warp * (CN / 4) + 2 * tig;
-#pragma unroll
-                for (int nt = 0; nt < NTW; ++nt) {
-                    const float v0 = gacc[nt][2 * h], v1 = gacc[nt][2 * h + 1];
-                    if (v0 != 0.f || v1 != 0.f) atomicAdd(reinterpret_cast<__nv_bfloat162*>(d + nt * 8), __floats2bfloat162_rn(v0, v1));
-                }
-            }
-#pragma unroll
-            for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
-                    const uint32_t row = p_base + (warp * 32 + mt * 16 + gid + 8 * h) * (BT_PSTR * 4);
+                    const int xp = x + gid + 8 * h;
+                    if (xp > bx1) continue;
+                    __nv_bfloat16* d = gs_b + ((long long)y * Ws + xp) * C + c0 + warp * (CN / 4) + 2 * tig;
 #pragma unroll
-                    for (int nt = 0; nt < 2; ++nt) {
-                        stsf(row + (nt * 8 + 2 * tig) * 4, pacc[mt][nt][2 * h]);
-                        stsf(row + (nt * 8 + 2 * tig + 1) * 4, pacc[mt][nt][2 * h + 1]);
+                    for (int nt = 0; nt < NTW; ++nt) {
+                        const float v0 = gacc[nt][2 * h], v1 = gacc[nt][2 * h + 1];
+                        if (v0 != 0.f || v1 != 0.f) atomicAdd(reinterpret_cast<__nv_bfloat162*>(d + nt * 8), __floats2bfloat162_rn(v0, v1));
                     }
                 }
-            __syncthreads();      // P of step s complete
-            if (regular) {
-                const uint32_t prow = p_base + tid * (BT_PSTR * 4);
 #pragma unroll
-                for (int r = 0; r < K1; ++r) {
-                    if (clampi(Y0u + r, Hs - 1) != y) continue;
+                for (int mt = 0; mt < 2; ++mt) {
+                    if (((pm >> mt) & 1u) == 0u) continue;      // nobody reads the P rows of inactive pixels
 #pragma unroll
-                    for (int t = 0; t < K1; ++t) {
-                        const int e = clampi(X0u + t, Ws - 1) - x;
-                        if (e >= 0 && e < SEG) Q[r * K1 + t] += ldsf(prow + e * 4);
+                    for (int h = 0; h < 2; ++h) {
+                        const uint32_t row = p_base + (warp * 32 + mt * 16 + gid + 8 * h) * (BT_PSTR * 4);
+#pragma unroll
+                        for (int nt = 0; nt < 2; ++nt) {
+                            stsf(row + (nt * 8 + 2 * tig) * 4, pacc[mt][nt][2 * h]);
+                            stsf(row + (nt * 8 + 2 * tig + 1) * 4, pacc[mt][nt][2 * h + 1]);
+                        }
+                    }
+                }
+                __syncthreads();      // P of step s complete
+                if (act) {
+                    const uint32_t prow = p_base + tid * (BT_PSTR * 4);
+#pragma unroll
+                    for (int r = 0; r < K1; ++r) {
+                        if (clampi(Y0u + r, Hs - 1) != y) continue;
+#pragma unroll
+                        for (int t = 0; t < K1; ++t) {
+                            const int e = clampi(X0u + t, Ws - 1) - x;
+                            if (e >= 0 && e < SEG) Q[r * K1 + t] += ldsf(prow + e * 4);
+                        }
                     }
                 }
             }
+            x = xn;
+            y = yn;
         }
     }
 

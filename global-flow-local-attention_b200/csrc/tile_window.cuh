@@ -64,10 +64,13 @@ __device__ __forceinline__ void group_bbox(const float* __restrict__ flow, int b
 // p = softmax probabilities (already scaled by whatever the caller wants, e.g. 1/k^2).  Border handling =
 // the reference's index clamp: weights of out-of-range columns / rows are folded onto the border position.
 // On return X0 / Y0 are shifted so that the mapping also holds for windows lying entirely outside the image.
+// The kernels only ever store the weights as bf16, so the window comes back as bf16 pairs: wp[r (K+1)/2 + s/2]
+// holds w[r][s] in its low half for even s, in its high half for odd s.
 template <int K>
 __device__ __forceinline__ void build_window(const float* p, const AxisTap<float> (&tx)[K], const AxisTap<float> (&ty)[K],
-                                             int Hs, int Ws, float scale, float* w, int& X0, int& Y0) {
+                                             int Hs, int Ws, float scale, uint32_t (&wp)[(K + 1) * (K + 1) / 2], int& X0, int& Y0) {
     constexpr int K1 = K + 1;
+    float w[K1 * K1];
 #pragma unroll
     for (int i = 0; i < K1 * K1; ++i) w[i] = 0.f;
 #pragma unroll
@@ -113,29 +116,48 @@ __device__ __forceinline__ void build_window(const float* p, const AxisTap<float
         X0 = min(max(X0, -K), Ws - 1);
         Y0 = min(max(Y0, -K), Hs - 1);
     }
+#pragma unroll
+    for (int i = 0; i < K1 * K1 / 2; ++i) wp[i] = bf16_bits(w[2 * i]) | (bf16_bits(w[2 * i + 1]) << 16);
 }
 
 // This pixel's weights for source row y, positions [x, x + SEG): window row y - Y0 (nothing when the row is outside the
 // window), stored as bf16 at base + e * stride for position x + e.  The zero entries are the caller's to write.
 template <int K>
-__device__ __forceinline__ void scatter_window_row(uint32_t base, uint32_t stride, const float* w, int X0, int Y0, int y, int x) {
-    constexpr int K1 = K + 1;
+__device__ __forceinline__ void scatter_window_row(uint32_t base, uint32_t stride, const uint32_t (&wp)[(K + 1) * (K + 1) / 2],
+                                                   int X0, int Y0, int y, int x) {
+    constexpr int K1 = K + 1, RW = K1 / 2;   // bf16 pairs per window row
     const int rr = y - Y0;
     if (rr < 0 || rr > K) return;
-    float wr[K1];
+    uint32_t wr[RW];
 #pragma unroll
-    for (int s = 0; s < K1; ++s) wr[s] = 0.f;
+    for (int s = 0; s < RW; ++s) wr[s] = 0u;
 #pragma unroll
     for (int r = 0; r < K1; ++r)
         if (rr == r) {
 #pragma unroll
-            for (int s = 0; s < K1; ++s) wr[s] = w[r * K1 + s];
+            for (int s = 0; s < RW; ++s) wr[s] = wp[r * RW + s];
         }
 #pragma unroll
     for (int s = 0; s < K1; ++s) {
         const int e = X0 + s - x;
-        if (e >= 0 && e < SEG && wr[s] != 0.f) sts16(base + e * stride, bf16_bits(wr[s]));
+        const uint32_t h = (s & 1) ? wr[s / 2] >> 16 : wr[s / 2] & 0xffffu;
+        if (e >= 0 && e < SEG && (h & 0x7fffu) != 0u) sts16(base + e * stride, h);
     }
+}
+
+// Does this pixel's window touch the step at source row y, positions [x, x + SEG)?  Its clamped extent
+// [clampi(X0), clampi(X0 + K)] x [clampi(Y0), clampi(Y0 + K)] is the same for the unfolded origin (tx[0].fl, ty[0].fl)
+// and the folded one build_window returns.  It holds every position scatter_window_row writes and every clamped position
+// the backward's Q pick reads, so a pixel for which this is false adds exact zeros to every MMA of the step.
+template <int K>
+__device__ __forceinline__ bool window_meets_step(int X0, int Y0, int Hs, int Ws, int y, int x) {
+    return clampi(Y0, Hs - 1) <= y && y <= clampi(Y0 + K, Hs - 1) && clampi(X0, Ws - 1) < x + SEG && clampi(X0 + K, Ws - 1) >= x;
+}
+
+// warp-collective: bit 0 = some pixel of group row 2 warp (lanes 0-15) is active, bit 1 = the same for row 2 warp + 1
+__device__ __forceinline__ uint32_t warp_row_bits(bool active) {
+    const uint32_t bal = __ballot_sync(0xffffffffu, active);
+    return ((bal & 0xffffu) != 0u ? 1u : 0u) | ((bal >> 16) != 0u ? 2u : 0u);
 }
 
 // One "irregular" pixel (taps not consecutive integers: fp32 rounding of (flow+offset)+coord straddling an integer,

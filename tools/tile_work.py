@@ -1,0 +1,122 @@
+"""Host-side count of the work the tensor-core tile kernels do on the bench workload (cfg2: B=16, 256x256, k=5, C=256),
+with and without skipping the MMA tiles of inactive 16-pixel group rows.
+
+    python tools/tile_work.py [--flow smooth|iid|both] [--seed N] [--B 16] [--H 256] [--W 256] [--k 5]
+
+Flows come from bench.py's two families (smooth = x16 bilinear up-sampling of U(-8,8), iid = U(-8,8)) drawn with their
+own seed, so these are statistics of the family, not of the bench's exact tensors.  The tap arithmetic is the kernels'
+(axis_tap in fp32, clamped windows), the footprint is group_bbox's and the steps are the kernels' row-major walk over
+16-position segments.  A pixel is active in a step when window_meets_step holds (tile_window.cuh); irregular pixels never are.
+
+Per-CTA-step costs (C = 256, warps of 32 pixels, mma.sync m16n8k16, ldmatrix .x4 = 512 B):
+  forward   4 passes of 64 channels; per warp and pass: 2 A + 4 B ldmatrix, 16 MMAs; skip: an inactive m-tile drops its
+            A ldmatrix and 8 MMAs, a warp without active pixels drops everything
+  backward  1 pass of 256 channels; P GEMM per warp: 16 k-steps x (2 A + 1 B) ldmatrix, 4 MMAs; GS GEMM per group row:
+            4 warps x (1 + 4) ldmatrix, 4 x 8 MMAs; skip: inactive m-tiles / group rows drop theirs, a step without any drops all
+"""
+import argparse
+
+import numpy as np
+
+SEG, GW, GH = 16, 16, 8
+LDSM = 512
+
+
+def make_flow(kind, B, H, W, seed):
+    import torch
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    if kind == "smooth":
+        coarse = torch.rand(B, 2, H // 16, W // 16, generator=g) * 16 - 8
+        flow = torch.nn.functional.interpolate(coarse, size=(H, W), mode="bilinear", align_corners=True)
+    else:
+        flow = torch.rand(B, 2, H, W, generator=g) * 16 - 8
+    return flow.float().numpy()
+
+
+def taps(flow, coord, k, dim):
+    """fl[j] = floor((flow + (j - k//2)) + coord) in fp32 (axis_tap), for j = 0..k-1"""
+    fl = [np.floor((flow + np.float32(j - k // 2)) + coord.astype(np.float32)).astype(np.int64) for j in range(k)]
+    regular = np.all([fl[j] == fl[0] + j for j in range(k)], axis=0)
+    lo = np.clip(fl[0], 0, dim - 1)
+    hi = np.clip(fl[k - 1] + 1, 0, dim - 1)
+    return fl[0], regular, lo, hi
+
+
+def count(flow, k):
+    B, _, H, W = flow.shape
+    ys, xs = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
+    X0, rx, bxlo, bxhi = taps(flow[:, 0], xs[None], k, W)
+    Y0, ry, bylo, byhi = taps(flow[:, 1], ys[None], k, H)
+    regular = rx & ry
+    cx0, cx1 = np.clip(X0, 0, W - 1), np.clip(X0 + k, 0, W - 1)
+    cy0, cy1 = np.clip(Y0, 0, H - 1), np.clip(Y0 + k, 0, H - 1)
+    inimg = np.ones((B, H, W), bool)
+    st = dict(groups=0, steps=[], entries=0, rows_on=0, warps_on=0, empty=0,
+              f_mma=[0, 0], f_ldsm=[0, 0], b_mma=[0, 0], b_ldsm=[0, 0])
+    for b in range(B):
+        for gy in range(0, H, GH):
+            for gx in range(0, W, GW):
+                sl = (b, slice(gy, gy + GH), slice(gx, gx + GW))
+                pad = lambda a, v: np.pad(a[sl], ((0, GH - a[sl].shape[0]), (0, GW - a[sl].shape[1])), constant_values=v).reshape(-1)
+                valid = pad(inimg, False)
+                bx0, bx1 = bxlo[sl].min(), bxhi[sl].max()
+                by0, by1 = bylo[sl].min(), byhi[sl].max()
+                sx = np.arange(bx0, bx1 + 1, SEG)
+                sy = np.arange(by0, by1 + 1)
+                y = np.repeat(sy, len(sx))[:, None]
+                x = np.tile(sx, len(sy))[:, None]
+                reg = pad(regular, False) & valid
+                a_x0, a_x1, a_y0, a_y1 = (pad(a, 0)[None] for a in (cx0, cx1, cy0, cy1))
+                act = reg[None] & (a_y0 <= y) & (y <= a_y1) & (a_x0 < x + SEG) & (a_x1 >= x)     # [steps, 128]
+                ent = np.clip(np.minimum(a_x1, x + SEG - 1) - np.maximum(a_x0, x) + 1, 0, None) * act
+                rows = act.reshape(len(y), 8, 16).any(axis=2)                                     # [steps, group rows]
+                n, nr = len(y), rows.sum(axis=1)
+                st["groups"] += 1
+                st["steps"].append(n)
+                st["entries"] += ent.sum()
+                st["rows_on"] += nr.sum()
+                st["warps_on"] += rows.reshape(n, 4, 2).any(axis=2).sum()
+                st["empty"] += (nr == 0).sum()
+                # forward, 4 passes x 4 warps
+                st["f_mma"][0] += 4 * n * 4 * 16
+                st["f_ldsm"][0] += 4 * n * 4 * 6 * LDSM
+                wtiles = rows.reshape(n, 4, 2)
+                st["f_mma"][1] += 4 * 8 * wtiles.sum()
+                st["f_ldsm"][1] += 4 * (wtiles.sum() + 4 * wtiles.any(axis=2).sum()) * LDSM
+                # backward, one pass of 256 channels
+                st["b_mma"][0] += n * (4 * 16 * 4 + 8 * 32)
+                st["b_ldsm"][0] += n * (4 * 16 * 3 + 8 * 20) * LDSM
+                st["b_mma"][1] += 16 * 2 * nr.sum() + 32 * nr.sum()
+                st["b_ldsm"][1] += (16 * (nr.sum() + wtiles.any(axis=2).sum()) + 20 * nr.sum()) * LDSM
+    return st
+
+
+def report(kind, st):
+    steps = np.array(st["steps"])
+    n = steps.sum()
+    print(f"== {kind} flow: {st['groups']} groups of 16x8 pixels")
+    print(f"steps per group (one pass)          mean {steps.mean():.1f}  p90 {np.percentile(steps, 90):.0f}  max {steps.max()}")
+    print(f"window entries in the dense slab    {100 * st['entries'] / (n * 128 * SEG):.1f} %")
+    print(f"active 16-pixel group rows          {100 * st['rows_on'] / (n * 8):.1f} %")
+    print(f"active warps (32 pixels)            {100 * st['warps_on'] / (n * 4):.1f} %")
+    print(f"steps without any active pixel      {100 * st['empty'] / n:.1f} %")
+    for name, m, l in (("forward", st["f_mma"], st["f_ldsm"]), ("backward", st["b_mma"], st["b_ldsm"])):
+        print(f"{name:9s} per CTA-step   MMAs {m[0] / n:7.1f} -> {m[1] / n:7.1f}   ldmatrix {l[0] / n / 1024:6.1f} KB -> {l[1] / n / 1024:6.1f} KB"
+              f"   ({100 * (1 - m[1] / m[0]):.0f} % / {100 * (1 - l[1] / l[0]):.0f} % skipped)")
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--flow", default="both", choices=["smooth", "iid", "both"])
+    ap.add_argument("--seed", type=int, default=1)
+    ap.add_argument("--B", type=int, default=16)
+    ap.add_argument("--H", type=int, default=256)
+    ap.add_argument("--W", type=int, default=256)
+    ap.add_argument("--k", type=int, default=5)
+    a = ap.parse_args()
+    for kind in (["smooth", "iid"] if a.flow == "both" else [a.flow]):
+        report(kind, count(make_flow(kind, a.B, a.H, a.W, a.seed), a.k))
+
+
+if __name__ == "__main__":
+    main()
