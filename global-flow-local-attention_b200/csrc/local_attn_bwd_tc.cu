@@ -7,12 +7,15 @@
 //     Q is exactly the CUDA-core kernel's Q (local_attn.cu), so grad_flow / grad_logits follow from it per pixel with
 //     the same formulas (local_attn_pixel.cuh);
 //   * GS[16 pos][CN] = Wfull^T[16 pos][128 px] * G[128 px][CN] grad_source of the segment, added with bf16x2 atomics
-//     (the caller's buffer is zero-filled first unless the call accumulates).
+//     (the caller's buffer is zero-filled first unless the call accumulates).  Border positions, where the windows
+//     folded onto the image edge pile up, are summed in an fp32 scratch instead and rounded once (k_fold_border).
 // The grad_out tile G stays in shared memory for the whole pass; the source segment arrives by cp.async one step ahead.
 // Warp w owns pixel rows 32w..32w+31 of the P GEMM and channels [w CN/4, (w+1) CN/4) of the GS GEMM (mma.sync m16n8k16).
 // A 16-pixel group row none of whose windows meets the step (window_meets_step) is skipped as a P m-tile and as a GS
 // k-step; the warps publish these row bits next to the step's weight slab.  Steps that no pixel touches do no MMAs.
 // Pixels whose taps are not consecutive integers take the reference's literal 4-tap arithmetic, one warp per pixel.
+#include <mutex>
+
 #include "tile_window.cuh"
 
 namespace gfla {
@@ -53,6 +56,18 @@ __device__ __forceinline__ void p_gemm(uint32_t ga, uint32_t sf, float (&pacc)[2
             mma_bf16(pacc[1][1], a1, bf[2], bf[3]);
         }
     }
+}
+
+// Slot of source position (y, x) on the image border (rows 0 and Hs-1, then columns 0 and Ws-1 of the rows between), in
+// [0, 2 (Hs + Ws)); -1 inside the image.  Windows folded onto the edge make border positions collect a share of nearly
+// every group of a border-clamped flow, and one bf16 atomic add per group would round each time.  Their grad_source is
+// summed in an fp32 buffer instead and rounded once by k_fold_border.
+__device__ __forceinline__ int border_slot(int y, int x, int Hs, int Ws) {
+    if (y == 0) return x;
+    if (y == Hs - 1) return Ws + x;
+    if (x == 0) return 2 * Ws + y;
+    if (x == Ws - 1) return 2 * Ws + Hs + y;
+    return -1;
 }
 
 template <int K>
@@ -109,7 +124,8 @@ template <int K, int CN>
 __global__ void __launch_bounds__(BT_THREADS, 1)
 k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow, const __nv_bfloat16* __restrict__ logits,
                     const __nv_bfloat16* __restrict__ gout, __nv_bfloat16* __restrict__ gsrc, float* __restrict__ gflow,
-                    __nv_bfloat16* __restrict__ glogits, int C, int Hs, int Ws, int H, int W, int gcols, int grows, int accumulate) {
+                    __nv_bfloat16* __restrict__ glogits, float* __restrict__ gborder, int C, int Hs, int Ws, int H, int W, int gcols,
+                    int grows, int accumulate) {
     constexpr int K1 = K + 1, KK = K * K;
     using L = BwdSmem<CN>;
     constexpr int GSTR = L::GSTR, NTW = CN / 32;
@@ -248,6 +264,16 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                 for (int h = 0; h < 2; ++h) {
                     const int xp = x + gid + 8 * h;
                     if (xp > bx1) continue;
+                    const int slot = border_slot(y, xp, Hs, Ws);
+                    if (slot >= 0) {
+                        float* d = gborder + ((long long)b * 2 * (Hs + Ws) + slot) * C + c0 + warp * (CN / 4) + 2 * tig;
+#pragma unroll
+                        for (int nt = 0; nt < NTW; ++nt) {
+                            const float v0 = gacc[nt][2 * h], v1 = gacc[nt][2 * h + 1];
+                            if (v0 != 0.f || v1 != 0.f) atomicAdd(reinterpret_cast<float2*>(d + nt * 8), make_float2(v0, v1));
+                        }
+                        continue;
+                    }
                     __nv_bfloat16* d = gs_b + ((long long)y * Ws + xp) * C + c0 + warp * (CN / 4) + 2 * tig;
 #pragma unroll
                     for (int nt = 0; nt < NTW; ++nt) {
@@ -311,9 +337,30 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     }
 }
 
+// grad_source of the border positions: what the buffer holds (the caller's values, plus the irregular pixels' adds) plus
+// the fp32 sum of the groups' adds, rounded once.  One thread per (image, border slot, channel pair).
+__global__ void __launch_bounds__(256)
+k_fold_border(__nv_bfloat16* __restrict__ gsrc, const float* __restrict__ gborder, int B, int C, int Hs, int Ws) {
+    const int nb = 2 * (Hs + Ws), c2 = C / 2;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)B * nb * c2) return;
+    const long long bs = i / c2;
+    const int c = (int)(i % c2) * 2, s = (int)(bs % nb), b = (int)(bs / nb);
+    int y, x;
+    if (s < Ws) { y = 0; x = s; }
+    else if (s < 2 * Ws) { y = Hs - 1; x = s - Ws; }
+    else if (s < 2 * Ws + Hs) { y = s - 2 * Ws; x = 0; }
+    else { y = s - 2 * Ws - Hs; x = Ws - 1; }
+    if (border_slot(y, x, Hs, Ws) != s) return;       // a slot no position maps to (a corner, or Hs or Ws of 1)
+    const float2 v = *reinterpret_cast<const float2*>(gborder + bs * C + c);
+    __nv_bfloat162* d = reinterpret_cast<__nv_bfloat162*>(gsrc + (((long long)b * Hs + y) * Ws + x) * C + c);
+    const float2 o = __bfloat1622float2(*d);
+    *d = __floats2bfloat162_rn(o.x + v.x, o.y + v.y);
+}
+
 template <int K, int CN>
 static int launch_bwd(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow, void* glogits,
-                      int B, int C, int Hs, int Ws, int H, int W, int accumulate, cudaStream_t st_) {
+                      float* gborder, int B, int C, int Hs, int Ws, int H, int W, int accumulate, cudaStream_t st_) {
     const int gcols = (W + GW - 1) / GW, grows = (H + GH - 1) / GH;
     const long long ngroups = (long long)B * gcols * grows;
     if (ngroups > INT_MAX) return GFLA_E_SHAPE;
@@ -322,11 +369,41 @@ static int launch_bwd(const void* src, const void* flow, const void* logits, con
     if (e != cudaSuccess) return static_cast<int>(e);
     kern<<<(unsigned)ngroups, BT_THREADS, BwdSmem<CN>::ALLOC, st_>>>(
         (const __nv_bfloat16*)src, (const float*)flow, (const __nv_bfloat16*)logits, (const __nv_bfloat16*)gout, (__nv_bfloat16*)gsrc,
-        (float*)gflow, (__nv_bfloat16*)glogits, C, Hs, Ws, H, W, gcols, grows, accumulate);
+        (float*)gflow, (__nv_bfloat16*)glogits, gborder, C, Hs, Ws, H, W, gcols, grows, accumulate);
+    const int st = launch_status();
+    if (st != GFLA_OK) return st;
+    const long long n = (long long)B * 2 * (Hs + Ws) * (C / 2);
+    k_fold_border<<<(unsigned)((n + 255) / 256), 256, 0, st_>>>((__nv_bfloat16*)gsrc, gborder, B, C, Hs, Ws);
     return launch_status();
 }
 
 }  // namespace tc
+
+// Stream-ordered scratch from a pool the library owns, one per device, that keeps its memory between calls: the device's
+// default pool hands its memory back at every synchronisation, and mapping it again each step costs more than the work.
+static cudaError_t scratch_alloc(void** p, size_t bytes, cudaStream_t st_) {
+    static std::mutex mu;
+    static cudaMemPool_t pools[64] = {};
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    if (dev >= 64) return cudaMallocAsync(p, bytes, st_);
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        if (pools[dev] == nullptr) {
+            cudaMemPoolProps props = {};
+            props.allocType = cudaMemAllocationTypePinned;
+            props.location.type = cudaMemLocationTypeDevice;
+            props.location.id = dev;
+            e = cudaMemPoolCreate(&pools[dev], &props);
+            if (e != cudaSuccess) { pools[dev] = nullptr; return e; }
+            uint64_t keep = UINT64_MAX;
+            e = cudaMemPoolSetAttribute(pools[dev], cudaMemPoolAttrReleaseThreshold, &keep);
+            if (e != cudaSuccess) return e;
+        }
+    }
+    return cudaMallocFromPoolAsync(p, bytes, pools[dev], st_);
+}
 
 static int pick_cn_bwd(int C) {
     if (C % 256 == 0) return 256;
@@ -349,12 +426,22 @@ int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, con
         if (z != GFLA_OK) return z;
     }
     const int cn = pick_cn_bwd(C);
+    if (cn == 0 || (k != 3 && k != 5)) return GFLA_E_NOTSUP;
+    // fp32 sums of the border positions' grad_source (border_slot), stream-ordered scratch
+    const size_t border_bytes = (size_t)B * 2 * (Hs + Ws) * C * sizeof(float);
+    float* gborder = nullptr;
+    cudaError_t e = scratch_alloc(reinterpret_cast<void**>(&gborder), border_bytes, st_);
+    if (e != cudaSuccess) return static_cast<int>(e);
+    int r = zero_async(gborder, border_bytes, st_);
+    if (r == GFLA_OK) {
 #define GFLA_BT_CASE(K_, CN_) \
-    if (k == K_ && cn == CN_) return tc::launch_bwd<K_, CN_>(src, flow, logits, gout, gsrc, gflow, glogits, B, C, Hs, Ws, H, W, accumulate, st_);
-    GFLA_BT_CASE(5, 256) GFLA_BT_CASE(5, 128) GFLA_BT_CASE(5, 64)
-    GFLA_BT_CASE(3, 256) GFLA_BT_CASE(3, 128) GFLA_BT_CASE(3, 64)
+        if (k == K_ && cn == CN_) r = tc::launch_bwd<K_, CN_>(src, flow, logits, gout, gsrc, gflow, glogits, gborder, B, C, Hs, Ws, H, W, accumulate, st_);
+        GFLA_BT_CASE(5, 256) GFLA_BT_CASE(5, 128) GFLA_BT_CASE(5, 64)
+        GFLA_BT_CASE(3, 256) GFLA_BT_CASE(3, 128) GFLA_BT_CASE(3, 64)
 #undef GFLA_BT_CASE
-    return GFLA_E_NOTSUP;
+    }
+    e = cudaFreeAsync(gborder, st_);
+    return r != GFLA_OK ? r : static_cast<int>(e);
 }
 
 }  // namespace gfla

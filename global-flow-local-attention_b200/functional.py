@@ -74,20 +74,27 @@ def block_extract_bwd(source, flow, grad_out, k, grad_source=None, grad_flow=Non
     _need_cuda(source, flow, grad_out)
     bs, ds, hs, ws = source.size()
     _, _, hf, wf = flow.size()
-    accumulate, narrow = 1, False
+    accumulate, narrow, flow_in = 1, False, flow
     if grad_source is None:
         accumulate = 0
         # 16-bit storage: scatter into an fp32 buffer (native red.global.f32; a 16-bit scalar atomicAdd is a
         # compare-and-swap loop, ~50x slower) and narrow afterwards
         narrow = source.dtype in (torch.bfloat16, torch.float16)
         grad_source = torch.empty(source.shape, dtype=torch.float32 if narrow else source.dtype, device=source.device)
-        grad_flow = torch.empty_like(flow)
+        # 16-bit flow: the kernel adds one partial grad_flow per channel slice, and in a 16-bit buffer each add would
+        # round.  Run on an fp32 copy of the flow (the kernel widens the flow to fp32 anyway, so the taps are the same)
+        # and round the gradient once.
+        if flow.dtype in (torch.bfloat16, torch.float16):
+            flow_in = convert(flow, torch.float32)
+        grad_flow = torch.empty_like(flow_in)
     with torch.cuda.device_of(source):
-        _lib.check(_lib.lib().gfla_block_extract_bwd(_p(source), _p(flow), _p(grad_out), _p(grad_source), _p(grad_flow),
-                                                     bs, ds, hs, ws, hf, wf, k, _dt(source), _dt(flow), _dt(grad_source),
+        _lib.check(_lib.lib().gfla_block_extract_bwd(_p(source), _p(flow_in), _p(grad_out), _p(grad_source), _p(grad_flow),
+                                                     bs, ds, hs, ws, hf, wf, k, _dt(source), _dt(flow_in), _dt(grad_source),
                                                      accumulate, _stream(source)), "block_extract_bwd")
     if narrow:
         grad_source = convert(grad_source, source.dtype)
+    if flow_in is not flow:
+        grad_flow = convert(grad_flow, flow.dtype)
     return grad_source, grad_flow
 
 

@@ -419,7 +419,7 @@ def test_local_attn_tile_vs_oracle(F_, oracle_lib, shape, kind, layout):
     np.testing.assert_allclose(host(probs), rprobs, rtol=0, atol=4e-3)
     np.testing.assert_allclose(host(out), ref, rtol=0, atol=1e-2)            # north_star tolerance
     # and much tighter than the contract against our own fp32-accumulating gather kernel:
-    # the only extra error is the bf16 rounding of the collapsed weights (2^-9 relative)
+    # the only extra error is the bf16 rounding of the collapsed weights (unit roundoff 2^-8, relative)
     g = F_.local_attn_fwd(s, f, l, k, algo="gather")
     err = (out.float() - g.float()).abs().max().item()
     assert err <= 3e-3, err
