@@ -6,13 +6,15 @@
 //     every position of the segment; each pixel thread then picks its (k+1)^2 window entries out of P into Q (registers).
 //     Q is exactly the CUDA-core kernel's Q (local_attn.cu), so grad_flow / grad_logits follow from it per pixel with
 //     the same formulas (local_attn_pixel.cuh);
-//   * GS[16 pos][CN] = Wfull^T[16 pos][128 px] * G[128 px][CN] grad_source of the segment, added with bf16x2 atomics
-//     (the caller's buffer is zero-filled first unless the call accumulates).  Border positions, where the windows
-//     folded onto the image edge pile up, are summed in an fp32 scratch instead and rounded once (k_fold_border).
+//   * GS[16 pos][CN] = Wfull^T[16 pos][128 px] * G[128 px][CN] grad_source of the segment, added with 16-byte bf16
+//     reductions (the caller's buffer is zero-filled first unless the call accumulates).  Border positions, where the
+//     windows folded onto the image edge pile up, are summed in an fp32 scratch instead and rounded once (k_fold_border).
 // The grad_out tile G stays in shared memory for the whole pass; the source segment arrives by cp.async one step ahead.
 // Warp w owns pixel rows 32w..32w+31 of the P GEMM and channels [w CN/4, (w+1) CN/4) of the GS GEMM (mma.sync m16n8k16).
 // A 16-pixel group row none of whose windows meets the step (window_meets_step) is skipped as a P m-tile and as a GS
 // k-step; the warps publish these row bits next to the step's weight slab.  Steps that no pixel touches do no MMAs.
+// One __syncthreads per step: a warp reads back only its own P rows, and the weight slab and its row bits rotate through
+// three buffers, so the slab a step zeroes was last read two steps earlier, before the previous step's barrier.
 // Pixels whose taps are not consecutive integers take the reference's literal 4-tap arithmetic, one warp per pixel.
 #include <mutex>
 
@@ -25,17 +27,37 @@ constexpr int BT_THREADS = 128;
 constexpr int BT_AWSTR = 128 * 2 + 16;          // transposed weight slab row (one position, 128 pixels) + pad
 constexpr int BT_PSTR = SEG + 1;                // P row (floats): odd stride, conflict-free per-pixel reads
 
+constexpr int BT_NAW = 3;                       // weight slabs (and row-bit words) in rotation
+
 template <int CN>
 struct BwdSmem {
     static constexpr int GSTR = CN * 2 + 16;
     static constexpr int G = 0;
     static constexpr int S = G + 128 * GSTR;
     static constexpr int AW = S + 2 * SEG * GSTR;
-    static constexpr int P = AW + 2 * SEG * BT_AWSTR;
+    static constexpr int P = AW + BT_NAW * SEG * BT_AWSTR;
     static constexpr int IRR = P + 128 * BT_PSTR * 4;
     static constexpr int ROWS = IRR + 129 * 4;      // per slab buffer: byte w = warp_row_bits of warp w for the step
-    static constexpr int ALLOC = ROWS + 2 * 4;
+    static constexpr int ALLOC = ROWS + BT_NAW * 4;
 };
+
+// 16-byte reduction: 8 bf16 values added element-wise, each add rounded once
+__device__ __forceinline__ void red_add_bf16x8(__nv_bfloat16* p, const uint32_t (&v)[4]) {
+    asm volatile("red.global.add.noftz.v4.bf16x2 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
+                 : "memory");
+}
+
+// 4x4 transpose of 32-bit words across the four lanes 4 g + t of a quad: on return lane t holds in v[n] what lane n held
+// in v[t].  Two butterfly rounds (lane distance 2, then 1), each trading two words.
+__device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int t) {
+    const bool t1 = (t & 2) != 0, t0 = (t & 1) != 0;
+    uint32_t y0 = __shfl_xor_sync(0xffffffffu, t1 ? v[0] : v[2], 2);
+    uint32_t y1 = __shfl_xor_sync(0xffffffffu, t1 ? v[1] : v[3], 2);
+    if (t1) { v[0] = y0; v[1] = y1; } else { v[2] = y0; v[3] = y1; }
+    y0 = __shfl_xor_sync(0xffffffffu, t0 ? v[0] : v[1], 1);
+    y1 = __shfl_xor_sync(0xffffffffu, t0 ? v[2] : v[3], 1);
+    if (t0) { v[0] = y0; v[2] = y1; } else { v[1] = y0; v[3] = y1; }
+}
 
 // P GEMM of one warp for one step: the m-tiles whose pixel row is active (M0, M1) of its 32 pixels x 16 positions
 template <int CN, bool M0, bool M1>
@@ -201,18 +223,20 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
         sts128(aw_base + (tid >> 3) * BT_AWSTR + (tid & 7) * 32 + 16, 0u, 0u, 0u, 0u);
         __syncthreads();          // slab 0 zeroed before anybody scatters into it
         // steps walk the footprint row-major: y from by0, x = bx0, bx0 + SEG, ... while x <= bx1
-        for (int s = 0, y = by0, x = bx0; y <= by1; ++s) {
-            const int buf = s & 1;
+        for (int s = 0, a = 0, y = by0, x = bx0; y <= by1; ++s) {
+            const int buf = s & 1;                      // source segment
+            const int an = a == BT_NAW - 1 ? 0 : a + 1;   // a = s % 3: weight slab and row bits; an: the next step's
             int xn = x + SEG, yn = y;
             if (xn > bx1) { xn = bx0; ++yn; }
-            const uint32_t aw = aw_base + buf * (SEG * BT_AWSTR);
-            // this pixel's column of Wfull^T for the segment (slab zeroed one step earlier); zero the other slab's share
+            const uint32_t aw = aw_base + a * (SEG * BT_AWSTR);
+            // this pixel's column of Wfull^T for the segment (slab zeroed one step earlier); zero this thread's share of the
+            // next step's slab, which step s-2 read before everybody passed the barrier of step s-1
             const bool act = regular && window_meets_step<K>(X0u, Y0u, Hs, Ws, y, x);
             if (act) scatter_window_row<K>(aw + tid * 2, BT_AWSTR, w, X0, Y0, y, x);
             {
                 const uint32_t rb = warp_row_bits(act);
-                if (lane == 0) rows[buf * 4 + warp] = static_cast<unsigned char>(rb);
-                const uint32_t z = aw_base + (buf ^ 1) * (SEG * BT_AWSTR) + (tid >> 3) * BT_AWSTR + (tid & 7) * 32;
+                if (lane == 0) rows[a * 4 + warp] = static_cast<unsigned char>(rb);
+                const uint32_t z = aw_base + an * (SEG * BT_AWSTR) + (tid >> 3) * BT_AWSTR + (tid & 7) * 32;
                 sts128(z, 0u, 0u, 0u, 0u);
                 sts128(z + 16, 0u, 0u, 0u, 0u);
             }
@@ -226,7 +250,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                 cp_async_commit();
             }
             // group rows with an active pixel: bit 8 v + h = group row 2 v + h (the same word in every thread)
-            const uint32_t grows_on = *reinterpret_cast<const uint32_t*>(rows + buf * 4);
+            const uint32_t grows_on = *reinterpret_cast<const uint32_t*>(rows + a * 4);
             if (grows_on != 0u) {
                 // P = G * S^T: this warp's 32 pixels x 16 positions, m-tiles of inactive pixel rows skipped
                 float pacc[2][2][4];
@@ -251,7 +275,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                 for (int kk = 0; kk < 128 / 16; ++kk) {
                     if (((grows_on >> (8 * (kk >> 1) + (kk & 1))) & 1u) == 0u) continue;
                     uint32_t af[4];
-                    ldsm_x4(aw_frag + buf * (SEG * BT_AWSTR) + kk * 32, af);
+                    ldsm_x4(aw_frag + a * (SEG * BT_AWSTR) + kk * 32, af);
 #pragma unroll
                     for (int np = 0; np < NTW / 2; ++np) {
                         uint32_t bg[4];
@@ -260,11 +284,15 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                         mma_bf16(gacc[2 * np + 1], af, bg[2], bg[3]);
                     }
                 }
+                // grad_source of the segment.  Positions past the footprint add nothing and border positions add fp32 pairs
+                // to the scratch.  The others are rounded to bf16 pairs, regrouped within each quad so that a lane holds 8
+                // consecutive channels of one position, and added 16 bytes at a time: per warp instruction, 8 positions x
+                // 64 contiguous bytes, two full 32-byte sectors each.
+                uint32_t gv[2 * NTW];       // [h NTW + nt]: channels nt 8 + 2 tig, +1 of position x + gid + 8 h, as bf16 pair
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const int xp = x + gid + 8 * h;
-                    if (xp > bx1) continue;
-                    const int slot = border_slot(y, xp, Hs, Ws);
+                    const int slot = xp > bx1 ? -2 : border_slot(y, xp, Hs, Ws);
                     if (slot >= 0) {
                         float* d = gborder + ((long long)b * 2 * (Hs + Ws) + slot) * C + c0 + warp * (CN / 4) + 2 * tig;
 #pragma unroll
@@ -272,13 +300,20 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                             const float v0 = gacc[nt][2 * h], v1 = gacc[nt][2 * h + 1];
                             if (v0 != 0.f || v1 != 0.f) atomicAdd(reinterpret_cast<float2*>(d + nt * 8), make_float2(v0, v1));
                         }
-                        continue;
                     }
-                    __nv_bfloat16* d = gs_b + ((long long)y * Ws + xp) * C + c0 + warp * (CN / 4) + 2 * tig;
 #pragma unroll
                     for (int nt = 0; nt < NTW; ++nt) {
-                        const float v0 = gacc[nt][2 * h], v1 = gacc[nt][2 * h + 1];
-                        if (v0 != 0.f || v1 != 0.f) atomicAdd(reinterpret_cast<__nv_bfloat162*>(d + nt * 8), __floats2bfloat162_rn(v0, v1));
+                        const __nv_bfloat162 v = __floats2bfloat162_rn(gacc[nt][2 * h], gacc[nt][2 * h + 1]);
+                        gv[h * NTW + nt] = slot == -1 ? *reinterpret_cast<const uint32_t*>(&v) : 0u;
+                    }
+                }
+#pragma unroll
+                for (int j = 0; j < NTW / 2; ++j) {
+                    uint32_t v[4] = {gv[4 * j], gv[4 * j + 1], gv[4 * j + 2], gv[4 * j + 3]};
+                    quad_transpose(v, tig);
+                    if ((v[0] | v[1] | v[2] | v[3]) != 0u) {        // all 8 values zero (or no position): nothing to add
+                        const int n = 4 * j + tig, h = n / NTW, nt = n % NTW;
+                        red_add_bf16x8(gs_b + ((long long)y * Ws + x + gid + 8 * h) * C + c0 + warp * (CN / 4) + nt * 8, v);
                     }
                 }
 #pragma unroll
@@ -294,7 +329,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                         }
                     }
                 }
-                __syncthreads();      // P of step s complete
+                __syncwarp();         // this warp's P rows of step s complete: they are the only rows its pixels read
                 if (act) {
                     const uint32_t prow = p_base + tid * (BT_PSTR * 4);
 #pragma unroll
@@ -310,6 +345,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
             }
             x = xn;
             y = yn;
+            a = an;
         }
     }
 

@@ -13,6 +13,16 @@ Per-CTA-step costs (C = 256, warps of 32 pixels, mma.sync m16n8k16, ldmatrix .x4
             A ldmatrix and 8 MMAs, a warp without active pixels drops everything
   backward  1 pass of 256 channels; P GEMM per warp: 16 k-steps x (2 A + 1 B) ldmatrix, 4 MMAs; GS GEMM per group row:
             4 warps x (1 + 4) ldmatrix, 4 x 8 MMAs; skip: inactive m-tiles / group rows drop theirs, a step without any drops all
+
+grad_source reductions of the backward, per CTA-step.  A position of the step receives a partial sum when some active
+pixel's clamped window covers it (every window entry is taken as nonzero).  Each warp adds its 64 channels of the
+16 positions, 8 positions (one half of the segment) per warp instruction:
+  bf16x2     (before) 8 instructions per warp and half with a covered position; each lane adds 4 B, so a position costs
+             one half-used 32-B sector per instruction: 32 sector operations per covered position
+  bf16x8     (now) the quad regroups its fragments so a lane holds 8 consecutive channels: 2 instructions per warp and
+             half, 64 contiguous bytes per position each, so 16 full-sector operations per covered position
+  fp32 pairs positions on the image border go to the fp32 scratch as before: 8 instructions per warp and half, one full
+             sector per position each
 """
 import argparse
 
@@ -52,7 +62,7 @@ def count(flow, k):
     cy0, cy1 = np.clip(Y0, 0, H - 1), np.clip(Y0 + k, 0, H - 1)
     inimg = np.ones((B, H, W), bool)
     st = dict(groups=0, steps=[], entries=0, rows_on=0, warps_on=0, empty=0,
-              f_mma=[0, 0], f_ldsm=[0, 0], b_mma=[0, 0], b_ldsm=[0, 0])
+              f_mma=[0, 0], f_ldsm=[0, 0], b_mma=[0, 0], b_ldsm=[0, 0], red_ins=[0, 0], red_sec=[0, 0], f32_ins=0, f32_sec=0)
     for b in range(B):
         for gy in range(0, H, GH):
             for gx in range(0, W, GW):
@@ -88,6 +98,19 @@ def count(flow, k):
                 st["b_ldsm"][0] += n * (4 * 16 * 3 + 8 * 20) * LDSM
                 st["b_mma"][1] += 16 * 2 * nr.sum() + 32 * nr.sum()
                 st["b_ldsm"][1] += (16 * (nr.sum() + wtiles.any(axis=2).sum()) + 20 * nr.sum()) * LDSM
+                # grad_source reductions: positions x + e of the step that an active pixel's window covers
+                pos = x + np.arange(SEG)[None]                                                    # [steps, 16]
+                cov = (act[:, None, :] & (a_x0[:, None, :] <= pos[:, :, None])
+                       & (pos[:, :, None] <= a_x1[:, None, :])).any(axis=2)
+                border = (y == 0) | (y == H - 1) | (pos == 0) | (pos == W - 1)
+                inner, edge = cov & ~border, cov & border
+                halves, ehalves = inner.reshape(n, 2, 8).any(axis=2).sum(), edge.reshape(n, 2, 8).any(axis=2).sum()
+                st["red_ins"][0] += 4 * 8 * halves
+                st["red_ins"][1] += 4 * 2 * halves
+                st["red_sec"][0] += 32 * inner.sum()
+                st["red_sec"][1] += 16 * inner.sum()
+                st["f32_ins"] += 4 * 8 * ehalves
+                st["f32_sec"] += 32 * edge.sum()
     return st
 
 
@@ -103,6 +126,10 @@ def report(kind, st):
     for name, m, l in (("forward", st["f_mma"], st["f_ldsm"]), ("backward", st["b_mma"], st["b_ldsm"])):
         print(f"{name:9s} per CTA-step   MMAs {m[0] / n:7.1f} -> {m[1] / n:7.1f}   ldmatrix {l[0] / n / 1024:6.1f} KB -> {l[1] / n / 1024:6.1f} KB"
               f"   ({100 * (1 - m[1] / m[0]):.0f} % / {100 * (1 - l[1] / l[0]):.0f} % skipped)")
+    ri, rs = st["red_ins"], st["red_sec"]
+    print(f"grad_source per CTA-step  bf16 reductions {ri[0] / n:5.1f} -> {ri[1] / n:5.1f} warp instructions, "
+          f"{rs[0] / n:6.1f} -> {rs[1] / n:6.1f} sector operations (bf16x2 -> bf16x8)")
+    print(f"                          border fp32 pairs {st['f32_ins'] / n:5.1f} warp instructions, {st['f32_sec'] / n:6.1f} sector operations")
 
 
 def main():
