@@ -12,17 +12,19 @@ name ``gfla_b200``.  Public surface = the reference's own classes:
     ExtractorAttn                                  (base_function.py:790-818)
     AffineRegularizationLoss / MultiAffineRegularizationLoss   (external_function.py:12-77)
     PerceptualCorrectness                          (external_function.py:222-284, on the fused Resample2dCosine op)
-plus the fused op ``local_attention`` / ``LocalAttnFunction`` and
-``compat.install()`` for the legacy extension-module names.
+plus the fused ops ``local_attention`` / ``LocalAttnFunction`` and ``patch_conv`` / ``PatchConvFunction``
+(ExtractorAttn's source-half conv without the block tensor), and ``compat.install()`` for the legacy
+extension-module names.
 """
 from .block_extractor import BlockExtractor, BlockExtractorFunction
-from .extractor_attn import ExtractorAttn, LocalAttnFunction, local_attention
+from .extractor_attn import ExtractorAttn, LocalAttnFunction, PatchConvFunction, local_attention, patch_conv
 from .local_attn_reshape import LocalAttnReshape, LocalAttnReshapeFunction
 from .losses import AffineRegularizationLoss, MultiAffineRegularizationLoss, PerceptualCorrectness
 from .resample2d import Resample2d, Resample2dCosine, Resample2dCosineFunction, Resample2dFunction
 from . import compat, functional, losses, sharding  # noqa: F401
 
 __all__ = ["BlockExtractor", "BlockExtractorFunction", "LocalAttnReshape", "LocalAttnReshapeFunction", "Resample2d",
-           "Resample2dFunction", "ExtractorAttn", "LocalAttnFunction", "local_attention", "AffineRegularizationLoss",
+           "Resample2dFunction", "ExtractorAttn", "LocalAttnFunction", "local_attention", "PatchConvFunction", "patch_conv",
+           "AffineRegularizationLoss",
            "MultiAffineRegularizationLoss", "PerceptualCorrectness", "Resample2dCosine", "Resample2dCosineFunction", "compat", "functional",
            "sharding"]

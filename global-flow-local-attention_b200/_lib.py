@@ -40,6 +40,8 @@ SIGNATURES = {
     "gfla_local_attn_bwd": [_vp] * 7 + [_i] * 12 + [_vp],
     "gfla_local_attn_bwd_workspace_bytes": [_i],
     "gfla_local_attn_bwd_ws": [_vp] * 7 + [_i] * 12 + [_vp, ctypes.c_longlong, _vp],
+    "gfla_patch_conv_fwd": [_vp] * 4 + [_i] * 11 + [_vp],
+    "gfla_patch_conv_bwd": [_vp] * 7 + [_i] * 12 + [_vp],
 }
 
 _lib = None

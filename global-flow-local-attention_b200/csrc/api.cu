@@ -20,6 +20,10 @@ int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, con
 int local_attn_fwd_tc(const void*, const void*, const void*, void*, void*, const void*, const void*, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
 int relayout(const void*, void*, int, int, int, int, int, int, cudaStream_t);
 bool local_attn_fwd_tc_supported(int C, int Ws, int k, int dtype, int flow_dtype, int layout, const void* src, const void* out);
+bool patch_conv_supported(int C, int N, int dtype, int flow_dtype, int layout);
+int patch_conv_fwd(const void*, const void*, const void*, void*, int, int, int, int, int, int, int, cudaStream_t);
+int patch_conv_bwd(const void*, const void*, const void*, const void*, void*, void*, void*, int, int, int, int, int, int, int, int,
+                   cudaStream_t);
 }  // namespace gfla
 
 #include <atomic>
@@ -226,6 +230,40 @@ int gfla_local_attn_bwd(const void* source, const void* flow, const void* logits
                                  (cudaStream_t)stream);
     return local_attn_bwd_gather(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W,
                                  k, dtype, flow_dtype, accumulate, layout, (cudaStream_t)stream);
+}
+
+// shape, dtype and support checks shared by the two patch-convolution entry points
+static int patch_conv_args(int B, int C, int Hs, int Ws, int H, int W, int k, int N, int dtype, int flow_dtype, int layout) {
+    if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
+    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || !pos(N) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    if (dtype != GFLA_BF16 || flow_dtype != GFLA_F32) return GFLA_E_DTYPE;
+    if (!patch_conv_supported(C, N, dtype, flow_dtype, layout)) return GFLA_E_NOTSUP;
+    return GFLA_OK;
+}
+
+int gfla_patch_conv_fwd(const void* source, const void* flow, const void* weight, void* out, int B, int C, int Hs, int Ws, int H,
+                        int W, int k, int N, int dtype, int flow_dtype, int layout, gfla_stream_t stream) {
+    REQ_PTR(source); REQ_PTR(flow); REQ_PTR(weight); REQ_PTR(out);
+    const int e = patch_conv_args(B, C, Hs, Ws, H, W, k, N, dtype, flow_dtype, layout);
+    if (e != GFLA_OK) return e;
+    if (!aligned(source, 16) || !aligned(weight, 16) || !aligned(out, 16)) return GFLA_E_ALIGN;
+    REQ_ALIGN(flow, flow_dtype);
+    return patch_conv_fwd(source, flow, weight, out, B, C, Hs, Ws, H, W, k, (cudaStream_t)stream);
+}
+
+int gfla_patch_conv_bwd(const void* source, const void* flow, const void* weight, const void* grad_out, void* grad_source_f32,
+                        void* grad_flow, void* grad_weight_f32, int B, int C, int Hs, int Ws, int H, int W, int k, int N, int dtype,
+                        int flow_dtype, int layout, int accumulate, gfla_stream_t stream) {
+    REQ_PTR(source); REQ_PTR(flow); REQ_PTR(weight); REQ_PTR(grad_out);
+    REQ_PTR(grad_source_f32); REQ_PTR(grad_flow); REQ_PTR(grad_weight_f32);
+    const int e = patch_conv_args(B, C, Hs, Ws, H, W, k, N, dtype, flow_dtype, layout);
+    if (e != GFLA_OK) return e;
+    if (!aligned(source, 16) || !aligned(weight, 16) || !aligned(grad_out, 16) || !aligned(grad_source_f32, 16) ||
+        !aligned(grad_weight_f32, 16))
+        return GFLA_E_ALIGN;
+    REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
+    return patch_conv_bwd(source, flow, weight, grad_out, grad_source_f32, grad_flow, grad_weight_f32, B, C, Hs, Ws, H, W, k,
+                          accumulate, (cudaStream_t)stream);
 }
 
 long long gfla_local_attn_bwd_workspace_bytes(int B) { (void)B; return 0; }   // the tile backward needs no workspace

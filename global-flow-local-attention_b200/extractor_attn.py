@@ -7,7 +7,8 @@ unchanged; what changes is how ``forward`` runs:
 
     reference                                   here
     ---------                                   ----
-    block_source = extractor(source, flow)      same (needed as conv input)
+    block_source = extractor(source, flow)      NOT materialised (softmax variant): its conv is patch_conv, an
+                                                implicit GEMM that gathers the bilinear taps itself
     block_target = extractor(target, 0)         NOT materialised: its conv == a stride-1 conv of `target`
                                                 with replicate padding (see _logits)
     attn = fc(cat(block_target, block_source))  conv -> act -> conv produce LOGITS;
@@ -69,6 +70,37 @@ def local_attention(source, flow_field, logits, kernel_size, algo="auto"):
                                    kernel_size, algo)
 
 
+class PatchConvFunction(Function):
+    """(source [B,C,Hs,Ws], flow [B,2,H,W] fp32, weight [128,C,k,k]) -> out [B,128,H,W]
+
+    out = conv2d(BlockExtractor(k)(source, flow), weight, None, stride=k), on the patch-convolution kernels: the taps are
+    gathered inside the GEMM, so neither the [B,C,kH,kW] block tensor nor its gradient is written.
+    """
+
+    @staticmethod
+    def forward(ctx, source, flow_field, weight, kernel_size):
+        ctx.save_for_backward(source, flow_field, weight)
+        ctx.kernel_size = kernel_size
+        return F_.patch_conv_fwd(source, flow_field, weight, kernel_size)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        source, flow_field, weight = ctx.saved_tensors
+        gs, gf, gw = F_.patch_conv_bwd(source, flow_field, weight, grad_output, ctx.kernel_size)
+        return gs, gf, gw, None
+
+
+def patch_conv(source, flow_field, weight, kernel_size):
+    """conv2d(BlockExtractor(kernel_size)(source, flow_field), weight, None, stride=kernel_size): the source half of
+    ExtractorAttn's first conv (base_function.py:800,805,807).  The kernels serve bf16 sources (channels-last, or NCHW
+    re-laid), C % 64 == 0 and 128 output channels; every other call runs that literal composition."""
+    src = _keep_format(source)
+    flow32 = _flow_f32(src, flow_field).contiguous()
+    if F_.patch_conv_eligible(src, flow32, weight, kernel_size):
+        return PatchConvFunction.apply(src, flow32, weight, kernel_size)
+    return F.conv2d(BlockExtractor(kernel_size)(source, flow_field), weight, None, stride=kernel_size)
+
+
 class ExtractorAttn(nn.Module):
     """Drop-in for base_function.py:790-818 (same ctor, same parameters)."""
 
@@ -87,19 +119,24 @@ class ExtractorAttn(nn.Module):
             nn.Conv2d(hidden_nc, kernel_size * kernel_size, kernel_size=1, stride=1, padding=0),
             softmax,)
 
-    def _logits(self, source, target, flow_field):
+    def _logits(self, source, target, flow_field, materialise=False):
         """conv(k, stride k) over cat(block_target, block_source), then act, then the 1x1 conv (no softmax).
 
         The target half never needs its block tensor: BlockExtractor with a zero flow copies, for output
         position (y*k+i, x*k+j), target[clamp(y+i-k//2), clamp(x+j-k//2)] (integer taps: weights 1 and 0,
         block_extractor_kernel.cu:62-82), so a kernel-k stride-k convolution over it IS an ordinary kernel-k
         stride-1 convolution of `target` with replicate padding (k//2 before, k-1-k//2 after) using the first
-        C input channels of the same weight.  Only block_source (flow-dependent, bilinear) is materialised.
+        C input channels of the same weight.  The source half is patch_conv, which gathers the bilinear taps
+        inside its GEMM; block_source is materialised (and returned) only when `materialise` asks for it.
         """
         conv1 = self.fully_connect_layer[0]
         k, c = self.kernel_size, source.shape[1]
-        block_source = self.extractor(source, flow_field)
-        x = F.conv2d(block_source, conv1.weight[:, c:], None, stride=k)
+        if materialise:
+            block_source = self.extractor(source, flow_field)
+            x = F.conv2d(block_source, conv1.weight[:, c:], None, stride=k)
+        else:
+            block_source = None
+            x = patch_conv(source, flow_field, conv1.weight[:, c:], k)
         lo, hi = k // 2, k - 1 - k // 2
         x = x + F.conv2d(F.pad(target, (lo, hi, lo, hi), mode="replicate"), conv1.weight[:, :c], conv1.bias)
         for layer in list(self.fully_connect_layer)[1:-1]:      # nonlinearity, 1x1 conv; not the softmax
@@ -110,7 +147,7 @@ class ExtractorAttn(nn.Module):
         """Reference signature (source, target, flow_field).  Optional `mask` [B,1,H,W]: also apply the caller's
         blend `target*(1-mask) + result*mask` (generator.py:130) -- fused into the kernel's store when no
         gradient is needed (inference), composed with torch ops otherwise."""
-        logits, block_source = self._logits(source, target, flow_field)
+        logits, block_source = self._logits(source, target, flow_field, materialise=not self.fused_softmax)
         if self.fused_softmax:
             if mask is None:
                 return local_attention(source, flow_field, logits, self.kernel_size)
@@ -128,7 +165,7 @@ class ExtractorAttn(nn.Module):
         return torch.nn.functional.avg_pool2d(attn_param * block_source, self.kernel_size, self.kernel_size)
 
     def hook_attn_param(self, source, target, flow_field):
-        logits, block_source = self._logits(source, target, flow_field)
+        logits, block_source = self._logits(source, target, flow_field, materialise=not self.fused_softmax)
         if self.fused_softmax:
             result, probs = F_.local_attn_fwd(_keep_format(source), _flow_f32(source, flow_field).contiguous(), logits.contiguous(),
                                               self.kernel_size, return_probs=True)

@@ -268,6 +268,71 @@ def relayout(t: torch.Tensor, to_channels_last: bool) -> torch.Tensor:
     return out
 
 
+# --------------------------------------------------------------------------- patch convolution
+PATCH_CONV_N = 128
+
+
+def patch_conv_eligible(source, flow, weight, k) -> bool:
+    """what the patch-convolution kernels serve (mirrors patch_conv_supported in csrc/patch_conv_tc.cu; an NCHW source
+    is re-laid to channels-last here)"""
+    return (source.is_cuda and source.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16
+            and flow.dtype == torch.float32 and source.dim() == 4 and source.shape[1] % 64 == 0
+            and tuple(weight.shape) == (PATCH_CONV_N, source.shape[1], k, k) and 1 <= k <= 9)
+
+
+def _pack_weight(weight):
+    """[N,C,k,k] -> [N][k][k][C] storage (what a channels_last weight already holds: then no copy)"""
+    return weight.permute(0, 2, 3, 1).contiguous()
+
+
+def patch_conv_fwd(source, flow, weight, k):
+    """out = conv2d(BlockExtractor(k)(source, flow), weight, None, stride=k) [B,128,H,W] without the block tensor, in the
+    source's memory format.  Only for calls patch_conv_eligible accepts."""
+    assert flow.is_contiguous()
+    _need_cuda(source, flow, weight)
+    planar = _feature_layout(source) == _lib.GFLA_NCHW
+    src = relayout(source, True) if planar else source
+    bs, ds, hs, ws = source.size()
+    _, df, h, w = flow.size()
+    assert df == 2 and flow.shape[0] == bs
+    n = weight.shape[0]
+    wp = _pack_weight(weight)
+    out = torch.empty((bs, h, w, n), dtype=source.dtype, device=source.device)       # channels-last storage
+    with torch.cuda.device_of(source):
+        _lib.check(_lib.lib().gfla_patch_conv_fwd(_p(src), _p(flow), _p(wp), _p(out), bs, ds, hs, ws, h, w, k, n, _dt(source),
+                                                  _dt(flow), _lib.GFLA_NHWC, _stream(source)), "patch_conv_fwd")
+    out = out.permute(0, 3, 1, 2)
+    return relayout(out, False) if planar else out
+
+
+def patch_conv_bwd(source, flow, weight, grad_out, k):
+    """-> (grad_source, grad_flow, grad_weight).  grad_source and grad_weight are summed in fp32 buffers and rounded
+    once; grad_source comes back in the source's memory format, grad_weight channels-last."""
+    assert flow.is_contiguous()
+    _need_cuda(source, flow, weight, grad_out)
+    planar = _feature_layout(source) == _lib.GFLA_NCHW
+    src = relayout(source, True) if planar else source
+    if grad_out.is_contiguous(memory_format=torch.channels_last):
+        go = grad_out
+    else:
+        go = relayout(grad_out.contiguous(), True)
+    bs, ds, hs, ws = source.size()
+    _, _, h, w = flow.size()
+    n = weight.shape[0]
+    wp = _pack_weight(weight)
+    gs32 = torch.empty((bs, hs, ws, ds), dtype=torch.float32, device=source.device)   # channels-last storage
+    gw32 = torch.empty((n, k, k, ds), dtype=torch.float32, device=source.device)
+    gf = torch.empty_like(flow)
+    with torch.cuda.device_of(source):
+        _lib.check(_lib.lib().gfla_patch_conv_bwd(_p(src), _p(flow), _p(wp), _p(go), _p(gs32), _p(gf), _p(gw32), bs, ds, hs, ws,
+                                                  h, w, k, n, _dt(source), _dt(flow), _lib.GFLA_NHWC, 0, _stream(source)),
+                   "patch_conv_bwd")
+    gs = convert(gs32, source.dtype).permute(0, 3, 1, 2)
+    del gs32
+    gw = convert(gw32, weight.dtype).permute(0, 3, 1, 2)
+    return (relayout(gs, False) if planar else gs), gf, gw
+
+
 def _tile_bwd_eligible(source, flow, k) -> bool:
     """what the backward tile kernels serve (mirrors local_attn_bwd_tc_supported in csrc/local_attn_bwd_tc.cu)"""
     c = source.shape[1]

@@ -220,6 +220,30 @@ int gfla_local_attn_bwd_ws(const void* source, const void* flow, const void* log
                            int dtype, int flow_dtype, int layout, int accumulate, int algo,
                            void* workspace, long long workspace_bytes, gfla_stream_t stream);
 
+/* ------------------------------------------------------------------------ *
+ * patch convolution = the source half of ExtractorAttn's first conv
+ *   replaces, in ExtractorAttn.forward (base_function.py:800,805,807),
+ *       block_source = BlockExtractor(k)(source, flow)                  # block_extractor_kernel.cu:20-85
+ *       conv2d(cat(block_target, block_source), W, stride=k)           # the input channels of block_source
+ *   and their backward (block_extractor_kernel.cu:89-170 + the conv's) by an implicit GEMM on the tensor cores:
+ *       out = conv2d(BlockExtractor(k)(source, flow), weight, None, stride=k)
+ *   computed without writing the [B,C,k*H,k*W] block tensor or its gradient.
+ *   source [B,C,Hs,Ws] channels-last (layout must be GFLA_NHWC); flow [B,2,H,W] planar;
+ *   weight [N][k][k][C] (the storage of a torch.channels_last [N,C,k,k] tensor); out [B,N,H,W] channels-last.
+ *   Served: dtype GFLA_BF16 with flow_dtype GFLA_F32, C % 64 == 0, N == 128 (GFLA_E_DTYPE / GFLA_E_NOTSUP otherwise).
+ *   source, weight, out, grad_out and the fp32 buffers must be 16-byte aligned.
+ *   Backward: grad_out [B,N,H,W] channels-last; grad_source_f32 [B,C,Hs,Ws] channels-last fp32 and
+ *   grad_weight_f32 [N][k][k][C] fp32 (narrow each with gfla_convert); grad_flow [B,2,H,W] fp32, written without
+ *   atomics (deterministic).  All three follow `accumulate`.
+ * ------------------------------------------------------------------------ */
+int gfla_patch_conv_fwd(const void* source, const void* flow, const void* weight, void* out,
+                        int B, int C, int Hs, int Ws, int H, int W, int k, int N,
+                        int dtype, int flow_dtype, int layout, gfla_stream_t stream);
+int gfla_patch_conv_bwd(const void* source, const void* flow, const void* weight, const void* grad_out,
+                        void* grad_source_f32, void* grad_flow, void* grad_weight_f32,
+                        int B, int C, int Hs, int Ws, int H, int W, int k, int N,
+                        int dtype, int flow_dtype, int layout, int accumulate, gfla_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

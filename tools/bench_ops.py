@@ -62,6 +62,51 @@ if "cfg2_fp32" in which:   # fused op in fp32 (CUDA-core gather kernels), B=4
     t = timed(lambda: F_.local_attn_bwd(s, fl, l, g, k), n=2, w=1)
     emit("local_attn_bwd fp32 (gather kernel, scalar atomics)", t, px, px * (3 * C * 4 + 16 + 2 * k * k * 4), config="B=4 C=256 256x256 k=5")
 
+if "patch_conv" in which:   # ExtractorAttn's source-half conv: materialised (BlockExtractor + cuDNN) vs patch_conv, bf16 channels-last
+    import subprocess
+    import gfla_b200
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+    card = q.stdout.strip() or torch.cuda.get_device_name(0)
+    torch.backends.cudnn.allow_tf32 = False
+    for (B, C, HW, k) in ((8, 256, 32, 3), (8, 128, 64, 5), (2, 256, 256, 5)):
+        cl = torch.channels_last
+        src = torch.randn(B, C, HW, HW, device=dev).bfloat16().contiguous(memory_format=cl).requires_grad_()
+        flow = smooth(B, HW, HW).requires_grad_()
+        w = (torch.randn(128, C, k, k, device=dev) / (C * k * k) ** 0.5).bfloat16().requires_grad_()
+        g = torch.randn(B, 128, HW, HW, device=dev).bfloat16().contiguous(memory_format=cl)
+        ex = gfla_b200.BlockExtractor(k)
+        arms = {"materialised": lambda: torch.nn.functional.conv2d(ex(src, flow), w, None, stride=k),
+                "patch_conv": lambda: gfla_b200.patch_conv(src, flow, w, k)}
+        with torch.no_grad():
+            outs = {a: fn() for a, fn in arms.items()}
+        diff = (outs["patch_conv"].float() - outs["materialised"].float()).abs().max().item()
+        del outs
+        res = {a: {"fwd": [], "fwd_bwd": []} for a in arms}
+        for rep in range(5):                      # alternate the arms so that clocks and heat affect both alike
+            for a, fn in arms.items():
+                with torch.no_grad():
+                    res[a]["fwd"].append(timed(fn, n=5, w=2))
+                res[a]["fwd_bwd"].append(timed(lambda: fn().backward(g), n=3, w=1))
+        gflop = 2 * B * HW * HW * 128 * C * k * k / 1e9
+        for a, fn in arms.items():
+            src.grad = flow.grad = w.grad = None
+            torch.cuda.synchronize()
+            torch.cuda.reset_peak_memory_stats()
+            base = torch.cuda.memory_allocated()
+            fn().backward(g)
+            torch.cuda.synchronize()
+            peak = torch.cuda.max_memory_allocated() - base
+            f, fb = sorted(res[a]["fwd"])[2], sorted(res[a]["fwd_bwd"])[2]
+            print(json.dumps({"op": f"patch conv, {a}", "config": f"B={B} C={C} {HW}x{HW} k={k} N=128 bf16 channels_last",
+                              "fwd_ms": round(f, 4), "fwd_bwd_ms": round(fb, 4),
+                              "fwd_TFLOPs": round(gflop / f, 2), "fwd_bwd_TFLOPs": round(3 * gflop / fb, 2),
+                              "frac_of_989_TFLOPs_fwd_bwd": round(3 * gflop / fb / 989.0, 4),
+                              "peak_MB_above_inputs_fwd_bwd": round(peak / 2 ** 20, 1),
+                              "max_abs_diff_vs_materialised": diff, "card_and_power_limit": card,
+                              "timing": "CUDA events, median of 5 alternating rounds"}), flush=True)
+        del src, flow, w, g
+        torch.cuda.empty_cache()
+
 if "module" in which:   # ExtractorAttn at the shapes the pose generator uses (SURVEY.md section 3): fused module vs the literal op chain
     import gfla_b200
     for (C, HW, k) in ((256, 32, 3), (128, 64, 5)):
