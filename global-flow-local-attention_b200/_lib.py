@@ -42,6 +42,12 @@ SIGNATURES = {
     "gfla_local_attn_bwd_ws": [_vp] * 7 + [_i] * 12 + [_vp, ctypes.c_longlong, _vp],
     "gfla_patch_conv_fwd": [_vp] * 4 + [_i] * 11 + [_vp],
     "gfla_patch_conv_bwd": [_vp] * 7 + [_i] * 12 + [_vp],
+    "gfla_local_attn_bwd_det_workspace_bytes": [_i] * 7,
+    "gfla_local_attn_bwd_det": [_vp] * 7 + [_i] * 12 + [_vp, ctypes.c_longlong, _vp],
+    "gfla_block_extract_bwd_det_workspace_bytes": [_i] * 7,
+    "gfla_block_extract_bwd_det": [_vp] * 5 + [_i] * 10 + [_vp, ctypes.c_longlong, _vp],
+    "gfla_patch_conv_bwd_det_workspace_bytes": [_i] * 8,
+    "gfla_patch_conv_bwd_det": [_vp] * 7 + [_i] * 12 + [_vp, ctypes.c_longlong, _vp],
 }
 
 _lib = None
@@ -64,7 +70,9 @@ def lib() -> ctypes.CDLL:
             fn.argtypes = argtypes
             fn.restype = _i
         l.gfla_debug_launch_count.restype = ctypes.c_ulonglong
-        l.gfla_local_attn_bwd_workspace_bytes.restype = ctypes.c_longlong
+        for name in SIGNATURES:
+            if name.endswith("_workspace_bytes"):
+                getattr(l, name).restype = ctypes.c_longlong
         l.gfla_error_string.argtypes = [_i]
         l.gfla_error_string.restype = ctypes.c_char_p
         if l.gfla_abi_version() != ABI_VERSION:

@@ -1,6 +1,6 @@
 // extern "C" surface of libgfla_warp.so (declared in include/gfla_warp.h):
 // argument validation + dispatch; no state, no allocation.
-#include "common.cuh"
+#include "det_accum.cuh"
 
 namespace gfla {
 int block_extract_fwd(const void*, const void*, void*, int, int, int, int, int, int, int, int, int, cudaStream_t);
@@ -24,6 +24,14 @@ bool patch_conv_supported(int C, int N, int dtype, int flow_dtype, int layout);
 int patch_conv_fwd(const void*, const void*, const void*, void*, int, int, int, int, int, int, int, cudaStream_t);
 int patch_conv_bwd(const void*, const void*, const void*, const void*, void*, void*, void*, int, int, int, int, int, int, int, int,
                    cudaStream_t);
+int local_attn_bwd_gather_det(const void*, const void*, const void*, const void*, void*, void*, int, int, int, int, int, int, int, int, int,
+                              int, int, fx_t*, const int*, cudaStream_t);
+int local_attn_bwd_tc_det(const void*, const void*, const void*, const void*, void*, void*, int, int, int, int, int, int, int, int, fx_t*,
+                          const int*, cudaStream_t);
+int block_extract_bwd_det(const void*, const void*, const void*, void*, int, int, int, int, int, int, int, int, int, int, fx_t*, const int*,
+                          cudaStream_t);
+int patch_conv_bwd_det(const void*, const void*, const void*, const void*, void*, int, int, int, int, int, int, int, int, fx_t*, fx_t*,
+                       const int*, cudaStream_t);
 }  // namespace gfla
 
 #include <atomic>
@@ -264,6 +272,141 @@ int gfla_patch_conv_bwd(const void* source, const void* flow, const void* weight
     REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
     return patch_conv_bwd(source, flow, weight, grad_out, grad_source_f32, grad_flow, grad_weight_f32, B, C, Hs, Ws, H, W, k,
                           accumulate, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------ deterministic backward passes (det_accum.cuh)
+// The workspace of each: the fixed-point sums of every scattered output, the exponents and the maxima (fx_layout).
+static FxLayout la_det_layout(int B, int C, int Hs, int Ws) { return fx_layout((long long)B * C * Hs * Ws, B, B); }
+static FxLayout be_det_layout(int B, int C, int Hs, int Ws) { return fx_layout((long long)B * C * Hs * Ws, B, B); }
+static FxLayout pc_det_layout(int B, int C, int Hs, int Ws, int k, int N) {
+    return fx_layout((long long)B * Hs * Ws * C + (long long)N * k * k * C, B + 1, B + 2);
+}
+
+// NULL workspace: GFLA_E_NULL; not 16-byte aligned: GFLA_E_ALIGN; smaller than needed: GFLA_E_SHAPE
+static int ws_check(const void* ws, long long bytes, const FxLayout& l) {
+    if (ws == nullptr) return GFLA_E_NULL;
+    if (!aligned(ws, 16)) return GFLA_E_ALIGN;
+    if (bytes < 0 || (size_t)bytes < l.total) return GFLA_E_SHAPE;
+    return GFLA_OK;
+}
+
+#define FX_PARTS(ws, l) \
+    fx_t* sums = reinterpret_cast<fx_t*>(ws); \
+    int* exps = reinterpret_cast<int*>(static_cast<char*>(ws) + (l).exps); \
+    fx_t* amax = reinterpret_cast<fx_t*>(static_cast<char*>(ws) + (l).amax)
+
+long long gfla_local_attn_bwd_det_workspace_bytes(int B, int C, int Hs, int Ws, int H, int W, int k) {
+    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    return (long long)la_det_layout(B, C, Hs, Ws).total;
+}
+
+int gfla_local_attn_bwd_det(const void* source, const void* flow, const void* logits, const void* grad_out, void* grad_source,
+                            void* grad_flow, void* grad_logits, int B, int C, int Hs, int Ws, int H, int W, int k, int dtype,
+                            int flow_dtype, int layout, int accumulate, int algo, void* workspace, long long workspace_bytes,
+                            gfla_stream_t stream) {
+    if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
+    REQ_PTR(source); REQ_PTR(flow); REQ_PTR(logits); REQ_PTR(grad_out); REQ_PTR(grad_source); REQ_PTR(grad_flow); REQ_PTR(grad_logits);
+    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
+    if (algo < 0 || algo > 2) return GFLA_E_NOTSUP;
+    REQ_ALIGN(source, dtype); REQ_ALIGN(logits, dtype); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_source, dtype);
+    REQ_ALIGN(grad_logits, dtype); REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
+    const FxLayout l = la_det_layout(B, C, Hs, Ws);
+    const int w = ws_check(workspace, workspace_bytes, l);
+    if (w != GFLA_OK) return w;
+    // the tile kernel never writes grad_source here (fx_narrow does): its alignment must not change which kernel runs
+    const bool tc_ok = local_attn_bwd_tc_supported(C, k, dtype, flow_dtype, layout, source, grad_out, source);
+    if (algo == 2 && !tc_ok) return GFLA_E_NOTSUP;
+    const cudaStream_t st_ = (cudaStream_t)stream;
+    FX_PARTS(workspace, l);
+    int r = zero_async(workspace, l.total, st_);
+    if (r == GFLA_OK) r = fx_amax(grad_out, dtype, (long long)C * H * W, B, amax, st_);
+    // Bound of image b: every pixel spreads g_c times weights that sum to exactly 1/k^2 (softmax probabilities summing to
+    // 1, times bilinear weights summing to 1, times 1/k^2) over the source positions, so every grad_source element of the
+    // image is at most (H W / k^2) max|G_b| in magnitude, and so is the sum of the magnitudes of its partials.  The tile
+    // kernel rounds the weights to bf16 first: a factor of at most 1 + 2^-8, inside the margin (det_accum.cuh).
+    if (r == GFLA_OK) r = fx_exponents(amax, B, nullptr, (double)H * W / ((double)k * k), false, exps, st_);
+    if (r == GFLA_OK) {
+        if (algo == 2 || (algo == 0 && tc_ok))
+            r = local_attn_bwd_tc_det(source, flow, logits, grad_out, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, accumulate, sums,
+                                      exps, st_);
+        else
+            r = local_attn_bwd_gather_det(source, flow, logits, grad_out, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype,
+                                          flow_dtype, accumulate, layout, sums, exps, st_);
+    }
+    if (r == GFLA_OK)
+        r = fx_narrow(sums, exps, (long long)C * Hs * Ws, (long long)B * C * Hs * Ws, grad_source, dtype, accumulate, st_);
+    return r;
+}
+
+long long gfla_block_extract_bwd_det_workspace_bytes(int B, int C, int Hs, int Ws, int Hf, int Wf, int k) {
+    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(Hf) || !pos(Wf) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    return (long long)be_det_layout(B, C, Hs, Ws).total;
+}
+
+int gfla_block_extract_bwd_det(const void* source, const void* flow, const void* grad_out, void* grad_source, void* grad_flow,
+                               int B, int C, int Hs, int Ws, int Hf, int Wf, int k, int dtype, int flow_dtype, int accumulate,
+                               void* workspace, long long workspace_bytes, gfla_stream_t stream) {
+    REQ_PTR(source); REQ_PTR(flow); REQ_PTR(grad_out); REQ_PTR(grad_source); REQ_PTR(grad_flow);
+    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(Hf) || !pos(Wf) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
+    REQ_ALIGN(source, dtype); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_source, dtype);
+    REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
+    const FxLayout l = be_det_layout(B, C, Hs, Ws);
+    const int w = ws_check(workspace, workspace_bytes, l);
+    if (w != GFLA_OK) return w;
+    const cudaStream_t st_ = (cudaStream_t)stream;
+    FX_PARTS(workspace, l);
+    int r = zero_async(workspace, l.total, st_);
+    if (r == GFLA_OK) r = fx_amax(grad_out, dtype, (long long)C * k * Hf * k * Wf, B, amax, st_);
+    // Bound of image b: every grad_out element spreads bilinear weights that sum to 1 over 4 source positions of its
+    // channel, so a grad_source element collects at most the k^2 Hf Wf elements of its channel: k^2 Hf Wf max|G_b|.
+    if (r == GFLA_OK) r = fx_exponents(amax, B, nullptr, (double)k * k * Hf * Wf, false, exps, st_);
+    if (r == GFLA_OK)
+        r = block_extract_bwd_det(source, flow, grad_out, grad_flow, B, C, Hs, Ws, Hf, Wf, k, dtype, flow_dtype, accumulate, sums, exps,
+                                  st_);
+    if (r == GFLA_OK)
+        r = fx_narrow(sums, exps, (long long)C * Hs * Ws, (long long)B * C * Hs * Ws, grad_source, dtype, accumulate, st_);
+    return r;
+}
+
+long long gfla_patch_conv_bwd_det_workspace_bytes(int B, int C, int Hs, int Ws, int H, int W, int k, int N) {
+    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || !pos(N) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    return (long long)pc_det_layout(B, C, Hs, Ws, k, N).total;
+}
+
+int gfla_patch_conv_bwd_det(const void* source, const void* flow, const void* weight, const void* grad_out, void* grad_source,
+                            void* grad_flow, void* grad_weight, int B, int C, int Hs, int Ws, int H, int W, int k, int N, int dtype,
+                            int flow_dtype, int layout, int accumulate, void* workspace, long long workspace_bytes,
+                            gfla_stream_t stream) {
+    REQ_PTR(source); REQ_PTR(flow); REQ_PTR(weight); REQ_PTR(grad_out);
+    REQ_PTR(grad_source); REQ_PTR(grad_flow); REQ_PTR(grad_weight);
+    const int e = patch_conv_args(B, C, Hs, Ws, H, W, k, N, dtype, flow_dtype, layout);
+    if (e != GFLA_OK) return e;
+    if (!aligned(source, 16) || !aligned(weight, 16) || !aligned(grad_out, 16)) return GFLA_E_ALIGN;
+    REQ_ALIGN(grad_source, dtype); REQ_ALIGN(grad_weight, dtype); REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
+    const FxLayout l = pc_det_layout(B, C, Hs, Ws, k, N);
+    const int w = ws_check(workspace, workspace_bytes, l);
+    if (w != GFLA_OK) return w;
+    const cudaStream_t st_ = (cudaStream_t)stream;
+    FX_PARTS(workspace, l);
+    const long long n_src = (long long)B * Hs * Ws * C, n_w = (long long)N * k * k * C;
+    int r = zero_async(workspace, l.total, st_);
+    if (r == GFLA_OK) r = fx_amax(grad_out, dtype, (long long)H * W * N, B, amax, st_);     // amax[b] = max|G_b|
+    if (r == GFLA_OK) r = fx_amax(weight, dtype, n_w, 1, amax + B, st_);                   // amax[B] = max|W|
+    if (r == GFLA_OK) r = fx_amax(source, dtype, n_src, 1, amax + B + 1, st_);             // amax[B+1] = max|source|
+    // grad_source of image b: GA[p, tap, c] = sum_n G[p, n] W[n, tap, c] is at most N max|G_b| max|W|, and each (pixel,
+    // tap) spreads it with bilinear weights summing to 1, so an element collects at most k^2 H W N max|G_b| max|W|.
+    if (r == GFLA_OK) r = fx_exponents(amax, B, amax + B, (double)k * k * H * W * N, false, exps, st_);
+    // grad_weight, one exponent for the call: sum over b and p of G[b, p, n] A[b, p, tap, c], where A (a convex blend of
+    // source values rounded to bf16) is at most max|source|: B H W max|G| max|source|.
+    if (r == GFLA_OK) r = fx_exponents(amax, B, amax + B + 1, (double)B * H * W, true, exps + B, st_);
+    if (r == GFLA_OK)
+        r = patch_conv_bwd_det(source, flow, weight, grad_out, grad_flow, B, C, Hs, Ws, H, W, k, accumulate, sums, sums + n_src, exps,
+                               st_);
+    if (r == GFLA_OK) r = fx_narrow(sums, exps, (long long)Hs * Ws * C, n_src, grad_source, dtype, accumulate, st_);
+    if (r == GFLA_OK) r = fx_narrow(sums + n_src, exps + B, n_w, n_w, grad_weight, dtype, accumulate, st_);
+    return r;
 }
 
 long long gfla_local_attn_bwd_workspace_bytes(int B) { (void)B; return 0; }   // the tile backward needs no workspace

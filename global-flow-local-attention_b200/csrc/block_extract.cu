@@ -15,7 +15,7 @@
 //   * 64-bit indexing throughout (the reference's `int n` overflows at cfg2).
 // This translation unit is compiled with -fmad=false so that the fp32/fp64
 // forward is bit-identical to the (uncontracted) CPU oracle.
-#include "common.cuh"
+#include "det_accum.cuh"
 
 namespace gfla {
 
@@ -55,12 +55,14 @@ k_block_extract_fwd(const T* __restrict__ src, const TF* __restrict__ flow, T* _
 }
 
 // TG = storage type of grad_source: T, or float for 16-bit T (native fp32 red.global instead of the
-// compare-and-swap loop a 16-bit scalar atomicAdd turns into; the caller narrows the buffer afterwards)
-template <typename T, typename TF, typename TG>
+// compare-and-swap loop a 16-bit scalar atomicAdd turns into; the caller narrows the buffer afterwards).
+// DET: grad_source goes into the fixed-point sums gsum with the image's exponent fx_exp[b] (det_accum.cuh).
+template <typename T, typename TF, typename TG, bool DET = false>
 __global__ void __launch_bounds__(128)
 k_block_extract_bwd(const T* __restrict__ src, const TF* __restrict__ flow, const T* __restrict__ gout,
                     TG* __restrict__ gsrc, TF* __restrict__ gflow,
-                    int B, int C, int Hs, int Ws, int Hf, int Wf, int k, int c_per_slice, int slices) {
+                    int B, int C, int Hs, int Ws, int Hf, int Wf, int k, int c_per_slice, int slices, fx_t* __restrict__ gsum,
+                    const int* __restrict__ fx_exp) {
     using A = typename Acc<T>::type;
     const long long total = (long long)B * Hf * Wf;
     const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -74,21 +76,30 @@ k_block_extract_bwd(const T* __restrict__ src, const TF* __restrict__ flow, cons
     const A flow_x = static_cast<A>(ld(flow + foff)), flow_y = static_cast<A>(ld(flow + foff + fpl));
     const int c0 = blockIdx.y * c_per_slice, c1 = min(C, c0 + c_per_slice);
     A gy = static_cast<A>(0), gx = static_cast<A>(0);
+    using GS = std::conditional_t<DET, fx_t, TG>;
+    GS* gs_img;
+    double2 fsc = make_double2(0.0, 0.0);
+    if constexpr (DET) {
+        gs_img = gsum;
+        fsc = fx_scale(fx_exp[b]);
+    } else {
+        gs_img = gsrc;
+    }
     for (int i = 0; i < k; ++i) {
         const AxisTap<A> ty = axis_tap<A>(flow_y, i - k / 2, yf, Hs);
         for (int j = 0; j < k; ++j) {
             const AxisTap<A> tx = axis_tap<A>(flow_x, j - k / 2, xf, Ws);
             const int oLT = ty.lo * Ws + tx.lo, oRT = ty.lo * Ws + tx.hi, oLB = ty.hi * Ws + tx.lo, oRB = ty.hi * Ws + tx.hi;
             const T* s = src + ((long long)b * C + c0) * spl;
-            TG* gs = gsrc + ((long long)b * C + c0) * spl;
+            GS* gs = gs_img + ((long long)b * C + c0) * spl;
             const T* go = gout + ((long long)b * C + c0) * opl + (long long)(yf * k + i) * Wo + (xf * k + j);
             for (int c = c0; c < c1; ++c, s += spl, gs += spl, go += opl) {
                 const A g = ld(go);
                 const A vLT = ld(s + oLT), vRT = ld(s + oRT), vLB = ld(s + oLB), vRB = ld(s + oRB);
-                red_add(gs + oLT, g * tx.wlo * ty.wlo);
-                red_add(gs + oRT, g * tx.whi * ty.wlo);
-                red_add(gs + oLB, g * tx.wlo * ty.whi);
-                red_add(gs + oRB, g * tx.whi * ty.whi);
+                scatter_add<DET>(gs + oLT, g * tx.wlo * ty.wlo, fsc);
+                scatter_add<DET>(gs + oRT, g * tx.whi * ty.wlo, fsc);
+                scatter_add<DET>(gs + oLB, g * tx.wlo * ty.whi, fsc);
+                scatter_add<DET>(gs + oRB, g * tx.whi * ty.whi, fsc);
                 gy += g * (-tx.wlo * vLT - tx.whi * vRT + tx.wlo * vLB + tx.whi * vRB);
                 gx += g * (-ty.wlo * vLT - ty.whi * vLB + ty.wlo * vRT + ty.whi * vRB);
             }
@@ -155,17 +166,18 @@ static int launch_be_fwd(const void* src, const void* flow, void* out, int B, in
     return launch_status();
 }
 
-template <typename T, typename TF, typename TG>
+template <typename T, typename TF, typename TG, bool DET = false>
 static int launch_be_bwd(const void* src, const void* flow, const void* gout, void* gsrc, void* gflow, int B, int C,
-                         int Hs, int Ws, int Hf, int Wf, int k, cudaStream_t st_) {
+                         int Hs, int Ws, int Hf, int Wf, int k, cudaStream_t st_, fx_t* gsum = nullptr, const int* fx_exp = nullptr) {
     const long long total = (long long)B * Hf * Wf;
     const int threads = 128;
-    const int slices0 = channel_splits(total, C, threads);
+    // DET: one channel slice, so that every thread owns its grad_flow element whatever the SM count
+    const int slices0 = DET ? 1 : channel_splits(total, C, threads);
     const int cps = (C + slices0 - 1) / slices0;
     const int slices = (C + cps - 1) / cps;
     dim3 grid((unsigned)((total + threads - 1) / threads), (unsigned)slices);
-    k_block_extract_bwd<T, TF, TG><<<grid, threads, 0, st_>>>((const T*)src, (const TF*)flow, (const T*)gout, (TG*)gsrc,
-                                                         (TF*)gflow, B, C, Hs, Ws, Hf, Wf, k, cps, slices);
+    k_block_extract_bwd<T, TF, TG, DET><<<grid, threads, 0, st_>>>((const T*)src, (const TF*)flow, (const T*)gout, (TG*)gsrc,
+                                                              (TF*)gflow, B, C, Hs, Ws, Hf, Wf, k, cps, slices, gsum, fx_exp);
     return launch_status();
 }
 
@@ -187,6 +199,20 @@ int block_extract_bwd(const void* src, const void* flow, const void* gout, void*
     return dispatch_dtypes(dtype, flow_dtype, gs_dtype, [&](auto t, auto tf, auto tg) -> int {
         return launch_be_bwd<typename decltype(t)::type, typename decltype(tf)::type, typename decltype(tg)::type>(
             src, flow, gout, gsrc, gflow, B, C, Hs, Ws, Hf, Wf, k, st_);
+    });
+}
+
+// grad_source into the fixed-point sums gsum (zeroed, exponents in fx_exp: det_accum.cuh); grad_flow follows `accumulate`
+int block_extract_bwd_det(const void* src, const void* flow, const void* gout, void* gflow, int B, int C, int Hs, int Ws, int Hf,
+                          int Wf, int k, int dtype, int flow_dtype, int accumulate, fx_t* gsum, const int* fx_exp, cudaStream_t st_) {
+    if (!accumulate) {
+        const int e = zero_async(gflow, (size_t)B * 2 * Hf * Wf * elem_size(flow_dtype), st_);
+        if (e != GFLA_OK) return e;
+    }
+    return dispatch_dtypes(dtype, flow_dtype, dtype, [&](auto t, auto tf, auto) -> int {
+        using T = typename decltype(t)::type;
+        return launch_be_bwd<T, typename decltype(tf)::type, T, true>(src, flow, gout, nullptr, gflow, B, C, Hs, Ws, Hf, Wf, k, st_,
+                                                                      gsum, fx_exp);
     });
 }
 

@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cstdlib>
+
 #include "../../include/gfla_warp.h"
 
 namespace gfla {
@@ -74,12 +76,19 @@ inline int elem_size(int dtype) {
 }
 inline bool aligned(const void* p, int bytes) { return (reinterpret_cast<uintptr_t>(p) % bytes) == 0; }
 
+// GFLA_SM_COUNT (a positive integer) replaces the queried count in every launch heuristic: it lets one GPU run the launch
+// shapes another H100 variant would get (114-SM PCIe vs 132-SM SXM), e.g. to check that the deterministic mode does not
+// depend on them.
 inline int sm_count() {
     static int n = 0;  // immutable after first query; benign if raced
     if (n == 0) {
-        int dev = 0, v = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+        const char* env = std::getenv("GFLA_SM_COUNT");
+        int v = env ? std::atoi(env) : 0;
+        if (v <= 0) {
+            int dev = 0;
+            cudaGetDevice(&dev);
+            cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+        }
         n = v > 0 ? v : 148;
     }
     return n;

@@ -18,6 +18,7 @@
 //     4*k*k bilinear taps collapse into a (k+1)x(k+1) window whose weights are
 //     computed once per pixel and reused for every channel;
 //   * otherwise the pixel takes the literal 4-taps-per-(i,j) path.
+#include "det_accum.cuh"
 #include "local_attn_pixel.cuh"
 
 namespace gfla {
@@ -123,12 +124,14 @@ k_local_attn_fwd(const T* __restrict__ src, const TF* __restrict__ flow, const T
 //   d source += g[c] * Wc[r][s] / k^2                         scatter-add
 // so each source value is read once per (pixel, channel) and the flow / logits
 // gradients need no atomics at all.
+// DET: grad_source goes into the fixed-point sums gsum (det_accum.cuh) with the image's exponent fx_exp[b] instead.
 // ---------------------------------------------------------------------------
-template <typename T, typename TF, int K>
+template <typename T, typename TF, int K, bool DET = false>
 __global__ void __launch_bounds__(128)
 k_local_attn_bwd(const T* __restrict__ src, const TF* __restrict__ flow, const T* __restrict__ logits,
                  const T* __restrict__ gout, T* __restrict__ gsrc, TF* __restrict__ gflow, T* __restrict__ glogits,
-                 int B, int C, int Hs, int Ws, int H, int W, int k_rt, int accumulate, int nhwc) {
+                 int B, int C, int Hs, int Ws, int H, int W, int k_rt, int accumulate, int nhwc, fx_t* __restrict__ gsum,
+                 const int* __restrict__ fx_exp) {
     using A = typename Acc<T>::type;
     const int k = K ? K : k_rt, KK = k * k;
     const long long hw = (long long)H * W, total = (long long)B * hw;
@@ -145,7 +148,15 @@ k_local_attn_bwd(const T* __restrict__ src, const TF* __restrict__ flow, const T
     const long long sc = nhwc ? 1 : spl, oc = nhwc ? 1 : hw;   // element strides per channel
     const int sp = nhwc ? C : 1;                               // element stride per source position
     const T* s = src + (long long)b * C * spl;
-    T* gs = gsrc + (long long)b * C * spl;
+    using GS = std::conditional_t<DET, fx_t, T>;
+    GS* gs;
+    double2 fsc = make_double2(0.0, 0.0);
+    if constexpr (DET) {
+        gs = gsum + (long long)b * C * spl;
+        fsc = fx_scale(fx_exp[b]);
+    } else {
+        gs = gsrc + (long long)b * C * spl;
+    }
     const T* go = gout + (long long)b * C * hw + pofs * (nhwc ? C : 1);
     const A inv_kk = static_cast<A>(1) / static_cast<A>(KK);
 
@@ -185,7 +196,7 @@ k_local_attn_bwd(const T* __restrict__ src, const TF* __restrict__ flow, const T
                     for (int q = 0; q < K1; ++q) {
                         const int o = cy[r] + cx[q];
                         Q[r * K1 + q] += g * ld(s + o);
-                        red_add(gs + o, g * Wc[r * K1 + q]);
+                        scatter_add<DET>(gs + o, g * Wc[r * K1 + q], fsc);
                     }
             }
 #pragma unroll
@@ -206,17 +217,17 @@ k_local_attn_bwd(const T* __restrict__ src, const TF* __restrict__ flow, const T
                 const A pij = p[i * k + j] * inv_kk;
                 A qLT = 0, qRT = 0, qLB = 0, qRB = 0;
                 const T* sq = s;
-                T* gc = gs;
+                GS* gc = gs;
                 const T* goc = go;
 #pragma unroll 1   // rare path, k*k copies of this loop: unrolled, it would raise the register pressure of the whole kernel
                 for (int c = 0; c < C; ++c, sq += sc, gc += sc, goc += oc) {
                     const A g = ld(goc);
                     qLT += g * ld(sq + oLT); qRT += g * ld(sq + oRT); qLB += g * ld(sq + oLB); qRB += g * ld(sq + oRB);
                     const A gp = g * pij;
-                    red_add(gc + oLT, gp * (tx.wlo * ty.wlo));
-                    red_add(gc + oRT, gp * (tx.whi * ty.wlo));
-                    red_add(gc + oLB, gp * (tx.wlo * ty.whi));
-                    red_add(gc + oRB, gp * (tx.whi * ty.whi));
+                    scatter_add<DET>(gc + oLT, gp * (tx.wlo * ty.wlo), fsc);
+                    scatter_add<DET>(gc + oRT, gp * (tx.whi * ty.wlo), fsc);
+                    scatter_add<DET>(gc + oLB, gp * (tx.wlo * ty.whi), fsc);
+                    scatter_add<DET>(gc + oRB, gp * (tx.whi * ty.whi), fsc);
                 }
                 dp[i * k + j] = tap_backward<A>(tx, ty, pij, inv_kk, qLT, qRT, qLB, qRB, gfx, gfy);
             }
@@ -237,16 +248,24 @@ static int la_launch_fwd(const void* src, const void* flow, const void* logits, 
     return launch_status();
 }
 
-template <typename T, typename TF, int K>
+template <typename T, typename TF, int K, bool DET = false>
 static int la_launch_bwd(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc,
                          void* gflow, void* glogits, int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate,
-                         int nhwc, cudaStream_t st_) {
+                         int nhwc, cudaStream_t st_, fx_t* gsum = nullptr, const int* fx_exp = nullptr) {
     const long long total = (long long)B * H * W;
     const int threads = 128;
-    k_local_attn_bwd<T, TF, K><<<(unsigned)((total + threads - 1) / threads), threads, 0, st_>>>(
+    k_local_attn_bwd<T, TF, K, DET><<<(unsigned)((total + threads - 1) / threads), threads, 0, st_>>>(
         (const T*)src, (const TF*)flow, (const T*)logits, (const T*)gout, (T*)gsrc, (TF*)gflow, (T*)glogits, B, C, Hs,
-        Ws, H, W, k, accumulate, nhwc);
+        Ws, H, W, k, accumulate, nhwc, gsum, fx_exp);
     return launch_status();
+}
+
+template <typename T, typename TF, int K>
+static int la_launch_bwd_det(const void* src, const void* flow, const void* logits, const void* gout, void* gflow, void* glogits,
+                             int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate, int nhwc, fx_t* gsum,
+                             const int* fx_exp, cudaStream_t st_) {
+    return la_launch_bwd<T, TF, K, true>(src, flow, logits, gout, nullptr, gflow, glogits, B, C, Hs, Ws, H, W, k, accumulate, nhwc,
+                                         st_, gsum, fx_exp);
 }
 
 #define GFLA_K_DISPATCH(fn, ...)                       \
@@ -281,6 +300,19 @@ int local_attn_bwd_gather(const void* src, const void* flow, const void* logits,
         using T = typename decltype(t)::type;
         using TF = typename decltype(tf)::type;
         GFLA_K_DISPATCH(la_launch_bwd, src, flow, logits, gout, gsrc, gflow, glogits, B, C, Hs, Ws, H, W, k, accumulate, nhwc, st_)
+    });
+}
+
+// grad_source into the fixed-point sums gsum (zeroed, exponents in fx_exp: det_accum.cuh); grad_flow / grad_logits as above
+int local_attn_bwd_gather_det(const void* src, const void* flow, const void* logits, const void* gout, void* gflow, void* glogits,
+                              int B, int C, int Hs, int Ws, int H, int W, int k, int dtype, int flow_dtype, int accumulate,
+                              int layout, fx_t* gsum, const int* fx_exp, cudaStream_t st_) {
+    const int nhwc = layout == GFLA_NHWC;
+    return dispatch_dtypes(dtype, flow_dtype, dtype, [&](auto t, auto tf, auto) -> int {
+        using T = typename decltype(t)::type;
+        using TF = typename decltype(tf)::type;
+        GFLA_K_DISPATCH(la_launch_bwd_det, src, flow, logits, gout, gflow, glogits, B, C, Hs, Ws, H, W, k, accumulate, nhwc, gsum,
+                        fx_exp, st_)
     });
 }
 

@@ -18,6 +18,7 @@
 // Pixels whose taps are not consecutive integers take the reference's literal 4-tap arithmetic, one warp per pixel.
 #include <mutex>
 
+#include "det_accum.cuh"
 #include "tile_window.cuh"
 
 namespace gfla {
@@ -92,12 +93,13 @@ __device__ __forceinline__ int border_slot(int y, int x, int Hs, int Ws) {
     return -1;
 }
 
-template <int K>
+template <int K, bool DET>
 __device__ __forceinline__ void irregular_pixel_bwd(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow,
                                                     const __nv_bfloat16* __restrict__ logits, const __nv_bfloat16* __restrict__ gout,
                                                     __nv_bfloat16* __restrict__ gsrc, float* __restrict__ gflow,
                                                     __nv_bfloat16* __restrict__ glogits, int b, int C, int Hs, int Ws, int H, int W,
-                                                    int qx, int qy, int accumulate, int lane) {
+                                                    int qx, int qy, int accumulate, int lane, fx_t* __restrict__ gsum,
+                                                    double2 fsc) {
     constexpr int KK = K * K;
     const long long hw = (long long)H * W, qofs = (long long)qy * W + qx;
     const float fx = flow[(long long)b * 2 * hw + qofs], fy = flow[(long long)b * 2 * hw + hw + qofs];
@@ -105,7 +107,10 @@ __device__ __forceinline__ void irregular_pixel_bwd(const __nv_bfloat16* __restr
     pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + qofs, hw, KK, p);
     const float inv_kk = 1.0f / static_cast<float>(KK);
     const __nv_bfloat16* s = src + (long long)b * Hs * Ws * C;
-    __nv_bfloat16* gs = gsrc + (long long)b * Hs * Ws * C;
+    using GS = std::conditional_t<DET, fx_t, __nv_bfloat16>;
+    GS* gs;
+    if constexpr (DET) gs = gsum + (long long)b * Hs * Ws * C;
+    else gs = gsrc + (long long)b * Hs * Ws * C;
     const __nv_bfloat16* go = gout + ((long long)b * hw + qofs) * C;
     float gfx = 0.f, gfy = 0.f;
 #pragma unroll
@@ -125,10 +130,10 @@ __device__ __forceinline__ void irregular_pixel_bwd(const __nv_bfloat16* __restr
                 q[2] += g * __bfloat162float(s[oLB + c]);
                 q[3] += g * __bfloat162float(s[oRB + c]);
                 const float gp = g * pij;
-                red_add(gs + oLT + c, gp * (tx.wlo * ty.wlo));
-                red_add(gs + oRT + c, gp * (tx.whi * ty.wlo));
-                red_add(gs + oLB + c, gp * (tx.wlo * ty.whi));
-                red_add(gs + oRB + c, gp * (tx.whi * ty.whi));
+                scatter_add<DET>(gs + oLT + c, gp * (tx.wlo * ty.wlo), fsc);
+                scatter_add<DET>(gs + oRT + c, gp * (tx.whi * ty.wlo), fsc);
+                scatter_add<DET>(gs + oLB + c, gp * (tx.wlo * ty.whi), fsc);
+                scatter_add<DET>(gs + oRB + c, gp * (tx.whi * ty.whi), fsc);
             }
 #pragma unroll
             for (int t = 0; t < 4; ++t)
@@ -142,12 +147,15 @@ __device__ __forceinline__ void irregular_pixel_bwd(const __nv_bfloat16* __restr
                                                            gflow + (long long)b * 2 * hw + qofs, hw, accumulate);
 }
 
-template <int K, int CN>
+// DET: grad_source goes into the fixed-point sums gsum with the image's exponent fx_exp[b] (det_accum.cuh); gsrc and
+// gborder are unused.  Each quad regroups its fp32 values so that every u64 reduction instruction of a warp covers
+// 8 positions x 32 contiguous bytes: whole sectors.
+template <int K, int CN, bool DET = false>
 __global__ void __launch_bounds__(BT_THREADS, 1)
 k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow, const __nv_bfloat16* __restrict__ logits,
                     const __nv_bfloat16* __restrict__ gout, __nv_bfloat16* __restrict__ gsrc, float* __restrict__ gflow,
                     __nv_bfloat16* __restrict__ glogits, float* __restrict__ gborder, int C, int Hs, int Ws, int H, int W, int gcols,
-                    int grows, int accumulate) {
+                    int grows, int accumulate, fx_t* __restrict__ gsum, const int* __restrict__ fx_exp) {
     constexpr int K1 = K + 1, KK = K * K;
     using L = BwdSmem<CN>;
     constexpr int GSTR = L::GSTR, NTW = CN / 32;
@@ -200,6 +208,12 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     const __nv_bfloat16* go_b = gout + (long long)b * hw * C;
     const __nv_bfloat16* s_b = src + (long long)b * Hs * Ws * C;
     __nv_bfloat16* gs_b = gsrc + (long long)b * Hs * Ws * C;
+    fx_t* gx_b = nullptr;
+    double2 fsc = make_double2(0.0, 0.0);
+    if constexpr (DET) {
+        gx_b = gsum + (long long)b * Hs * Ws * C;
+        fsc = fx_scale(fx_exp[b]);
+    }
 
     for (int c0 = 0; c0 < C; c0 += CN) {
         __syncthreads();          // the previous pass is done with G, S and the weight slabs
@@ -284,36 +298,68 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                         mma_bf16(gacc[2 * np + 1], af, bg[2], bg[3]);
                     }
                 }
-                // grad_source of the segment.  Positions past the footprint add nothing and border positions add fp32 pairs
-                // to the scratch.  The others are rounded to bf16 pairs, regrouped within each quad so that a lane holds 8
-                // consecutive channels of one position, and added 16 bytes at a time: per warp instruction, 8 positions x
-                // 64 contiguous bytes, two full 32-byte sectors each.
-                uint32_t gv[2 * NTW];       // [h NTW + nt]: channels nt 8 + 2 tig, +1 of position x + gid + 8 h, as bf16 pair
+                if constexpr (DET) {
+                    // grad_source of the segment as fixed-point sums, no rounding of the partials and no border scratch.
+                    // Lane t of a quad holds channels 2t, 2t+1 of each 8-channel group nt.  Per pair of groups (2j, 2j+1):
+                    // the exchange with lane t^1 gives lane t the 4 consecutive channels 4 (t >> 1) .. +3 of group
+                    // 2j + (t & 1); the quad transpose then gives lane t channel 4 (n >> 1) + t of group 2j + (n & 1) in
+                    // word n, so the four lanes of a quad add one whole 32-byte sector per instruction.
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int xp = x + gid + 8 * h;
-                    const int slot = xp > bx1 ? -2 : border_slot(y, xp, Hs, Ws);
-                    if (slot >= 0) {
-                        float* d = gborder + ((long long)b * 2 * (Hs + Ws) + slot) * C + c0 + warp * (CN / 4) + 2 * tig;
+                    for (int h = 0; h < 2; ++h) {
+                        const int xp = x + gid + 8 * h;
+                        fx_t* d = gx_b + ((long long)y * Ws + xp) * C + c0 + warp * (CN / 4);
+                        const bool t0 = (tig & 1) != 0;
 #pragma unroll
-                        for (int nt = 0; nt < NTW; ++nt) {
-                            const float v0 = gacc[nt][2 * h], v1 = gacc[nt][2 * h + 1];
-                            if (v0 != 0.f || v1 != 0.f) atomicAdd(reinterpret_cast<float2*>(d + nt * 8), make_float2(v0, v1));
+                        for (int j = 0; j < NTW / 2; ++j) {
+                            const float a0 = gacc[2 * j][2 * h], a1 = gacc[2 * j][2 * h + 1];
+                            const float b0 = gacc[2 * j + 1][2 * h], b1 = gacc[2 * j + 1][2 * h + 1];
+                            const float r0 = __shfl_xor_sync(0xffffffffu, t0 ? a0 : b0, 1);
+                            const float r1 = __shfl_xor_sync(0xffffffffu, t0 ? a1 : b1, 1);
+                            uint32_t v[4];
+                            v[0] = __float_as_uint(t0 ? r0 : a0);
+                            v[1] = __float_as_uint(t0 ? r1 : a1);
+                            v[2] = __float_as_uint(t0 ? b0 : r0);
+                            v[3] = __float_as_uint(t0 ? b1 : r1);
+                            quad_transpose(v, tig);
+                            if (xp <= bx1) {
+#pragma unroll
+                                for (int n = 0; n < 4; ++n)
+                                    fx_add(d + (2 * j + (n & 1)) * 8 + 4 * (n >> 1) + tig, __uint_as_float(v[n]), fsc);
+                            }
                         }
                     }
-#pragma unroll
-                    for (int nt = 0; nt < NTW; ++nt) {
-                        const __nv_bfloat162 v = __floats2bfloat162_rn(gacc[nt][2 * h], gacc[nt][2 * h + 1]);
-                        gv[h * NTW + nt] = slot == -1 ? *reinterpret_cast<const uint32_t*>(&v) : 0u;
+                } else {
+                    // grad_source of the segment.  Positions past the footprint add nothing and border positions add fp32 pairs
+                    // to the scratch.  The others are rounded to bf16 pairs, regrouped within each quad so that a lane holds 8
+                    // consecutive channels of one position, and added 16 bytes at a time: per warp instruction, 8 positions x
+                    // 64 contiguous bytes, two full 32-byte sectors each.
+                    uint32_t gv[2 * NTW];       // [h NTW + nt]: channels nt 8 + 2 tig, +1 of position x + gid + 8 h, as bf16 pair
+    #pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int xp = x + gid + 8 * h;
+                        const int slot = xp > bx1 ? -2 : border_slot(y, xp, Hs, Ws);
+                        if (slot >= 0) {
+                            float* d = gborder + ((long long)b * 2 * (Hs + Ws) + slot) * C + c0 + warp * (CN / 4) + 2 * tig;
+    #pragma unroll
+                            for (int nt = 0; nt < NTW; ++nt) {
+                                const float v0 = gacc[nt][2 * h], v1 = gacc[nt][2 * h + 1];
+                                if (v0 != 0.f || v1 != 0.f) atomicAdd(reinterpret_cast<float2*>(d + nt * 8), make_float2(v0, v1));
+                            }
+                        }
+    #pragma unroll
+                        for (int nt = 0; nt < NTW; ++nt) {
+                            const __nv_bfloat162 v = __floats2bfloat162_rn(gacc[nt][2 * h], gacc[nt][2 * h + 1]);
+                            gv[h * NTW + nt] = slot == -1 ? *reinterpret_cast<const uint32_t*>(&v) : 0u;
+                        }
                     }
-                }
-#pragma unroll
-                for (int j = 0; j < NTW / 2; ++j) {
-                    uint32_t v[4] = {gv[4 * j], gv[4 * j + 1], gv[4 * j + 2], gv[4 * j + 3]};
-                    quad_transpose(v, tig);
-                    if ((v[0] | v[1] | v[2] | v[3]) != 0u) {        // all 8 values zero (or no position): nothing to add
-                        const int n = 4 * j + tig, h = n / NTW, nt = n % NTW;
-                        red_add_bf16x8(gs_b + ((long long)y * Ws + x + gid + 8 * h) * C + c0 + warp * (CN / 4) + nt * 8, v);
+    #pragma unroll
+                    for (int j = 0; j < NTW / 2; ++j) {
+                        uint32_t v[4] = {gv[4 * j], gv[4 * j + 1], gv[4 * j + 2], gv[4 * j + 3]};
+                        quad_transpose(v, tig);
+                        if ((v[0] | v[1] | v[2] | v[3]) != 0u) {        // all 8 values zero (or no position): nothing to add
+                            const int n = 4 * j + tig, h = n / NTW, nt = n % NTW;
+                            red_add_bf16x8(gs_b + ((long long)y * Ws + x + gid + 8 * h) * C + c0 + warp * (CN / 4) + nt * 8, v);
+                        }
                     }
                 }
 #pragma unroll
@@ -368,8 +414,8 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     // ---- pixels with non-consecutive taps: literal arithmetic, one warp per pixel
     for (int i = warp; i < nirr; i += BT_THREADS / 32) {
         const int m = irr[i];
-        irregular_pixel_bwd<K>(src, flow, logits, gout, gsrc, gflow, glogits, b, C, Hs, Ws, H, W, gx0 + (m & 15), gy0 + (m >> 4),
-                               accumulate, lane);
+        irregular_pixel_bwd<K, DET>(src, flow, logits, gout, gsrc, gflow, glogits, b, C, Hs, Ws, H, W, gx0 + (m & 15),
+                                    gy0 + (m >> 4), accumulate, lane, gsum, fsc);
     }
 }
 
@@ -394,20 +440,21 @@ k_fold_border(__nv_bfloat16* __restrict__ gsrc, const float* __restrict__ gborde
     *d = __floats2bfloat162_rn(o.x + v.x, o.y + v.y);
 }
 
-template <int K, int CN>
+template <int K, int CN, bool DET = false>
 static int launch_bwd(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow, void* glogits,
-                      float* gborder, int B, int C, int Hs, int Ws, int H, int W, int accumulate, cudaStream_t st_) {
+                      float* gborder, int B, int C, int Hs, int Ws, int H, int W, int accumulate, cudaStream_t st_,
+                      fx_t* gsum = nullptr, const int* fx_exp = nullptr) {
     const int gcols = (W + GW - 1) / GW, grows = (H + GH - 1) / GH;
     const long long ngroups = (long long)B * gcols * grows;
     if (ngroups > INT_MAX) return GFLA_E_SHAPE;
-    auto kern = k_local_attn_bwd_tc<K, CN>;
+    auto kern = k_local_attn_bwd_tc<K, CN, DET>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem<CN>::ALLOC);
     if (e != cudaSuccess) return static_cast<int>(e);
     kern<<<(unsigned)ngroups, BT_THREADS, BwdSmem<CN>::ALLOC, st_>>>(
         (const __nv_bfloat16*)src, (const float*)flow, (const __nv_bfloat16*)logits, (const __nv_bfloat16*)gout, (__nv_bfloat16*)gsrc,
-        (float*)gflow, (__nv_bfloat16*)glogits, gborder, C, Hs, Ws, H, W, gcols, grows, accumulate);
+        (float*)gflow, (__nv_bfloat16*)glogits, gborder, C, Hs, Ws, H, W, gcols, grows, accumulate, gsum, fx_exp);
     const int st = launch_status();
-    if (st != GFLA_OK) return st;
+    if (st != GFLA_OK || DET) return st;
     const long long n = (long long)B * 2 * (Hs + Ws) * (C / 2);
     k_fold_border<<<(unsigned)((n + 255) / 256), 256, 0, st_>>>((__nv_bfloat16*)gsrc, gborder, B, C, Hs, Ws);
     return launch_status();
@@ -478,6 +525,20 @@ int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, con
     }
     e = cudaFreeAsync(gborder, st_);
     return r != GFLA_OK ? r : static_cast<int>(e);
+}
+
+// grad_source into the fixed-point sums gsum (zeroed, channels-last, exponents in fx_exp: det_accum.cuh); no border scratch
+// and no k_fold_border.  grad_flow / grad_logits follow `accumulate` as above.
+int local_attn_bwd_tc_det(const void* src, const void* flow, const void* logits, const void* gout, void* gflow, void* glogits, int B,
+                          int C, int Hs, int Ws, int H, int W, int k, int accumulate, fx_t* gsum, const int* fx_exp, cudaStream_t st_) {
+    const int cn = pick_cn_bwd(C);
+#define GFLA_BT_CASE(K_, CN_) \
+    if (k == K_ && cn == CN_) return tc::launch_bwd<K_, CN_, true>(src, flow, logits, gout, nullptr, gflow, glogits, nullptr, B, C, Hs, Ws, \
+                                                                   H, W, accumulate, st_, gsum, fx_exp);
+    GFLA_BT_CASE(5, 256) GFLA_BT_CASE(5, 128) GFLA_BT_CASE(5, 64)
+    GFLA_BT_CASE(3, 256) GFLA_BT_CASE(3, 128) GFLA_BT_CASE(3, 64)
+#undef GFLA_BT_CASE
+    return GFLA_E_NOTSUP;
 }
 
 }  // namespace gfla

@@ -15,6 +15,7 @@
 // this step's MMAs run, with one __syncthreads per step.  mma.sync m16n8k16, bf16 in, fp32 accumulate.
 #include <climits>
 
+#include "det_accum.cuh"
 #include "tile_window.cuh"
 
 namespace gfla {
@@ -29,6 +30,7 @@ constexpr int PC_FSTR = PC_CK * 4 + 16;       // fp32 row of one chunk + pad: 27
 constexpr int PC_ABYTES = 128 * PC_ASTR;      // one [128][64] bf16 operand
 constexpr int PC_GBYTES = 128 * PC_GSTR;      // one [128][128] bf16 operand
 
+constexpr int PCW_DET_GROUPS = 256;           // pixel groups per weight-gradient slice in the deterministic mode
 constexpr int PCF_SMEM = 4 * PC_ABYTES;                            // forward: A and W_t, two buffers each
 constexpr int PCB_SMEM = PC_GBYTES + 2 * PC_ABYTES + 128 * PC_FSTR;  // backward: G, W_t x 2, GA (fp32)
 constexpr int PCW_SMEM = 2 * PC_GBYTES + 2 * PC_ABYTES;            // weight gradient: G x 2, A x 2
@@ -218,10 +220,13 @@ k_patch_conv_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
 // --------------------------------------------------------------------------------------------- backward: data gradients
 // Warp w computes GA rows 16 w .. +16 (all 64 channels of the chunk); its A fragments of G stay in registers for the whole
 // K loop.  Then every thread takes half a pixel row of GA, as in the forward's gather.
+// DET: grad_source goes into the fixed-point sums gsum (channels-last) with the image's exponent fx_exp[b] (det_accum.cuh).
+template <bool DET = false>
 __global__ void __launch_bounds__(PC_THREADS, 2)
 k_patch_conv_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow, const __nv_bfloat16* __restrict__ wpk,
                     const __nv_bfloat16* __restrict__ gout, float* __restrict__ gsrc, float* __restrict__ gflow, int C, int Hs,
-                    int Ws, int H, int W, int k, int gcols, int grows, int accumulate) {
+                    int Ws, int H, int W, int k, int gcols, int grows, int accumulate, fx_t* __restrict__ gsum,
+                    const int* __restrict__ fx_exp) {
     extern __shared__ __align__(16) unsigned char smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
     int b, gx0, gy0;
@@ -233,6 +238,12 @@ k_patch_conv_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     const float fx = valid ? flow[fofs] : 0.f, fy = valid ? flow[fofs + hw] : 0.f;
     const __nv_bfloat16* s_img = src + (long long)b * Hs * Ws * C;
     float* gs_img = gsrc + (long long)b * Hs * Ws * C;
+    fx_t* gx_img = nullptr;
+    double2 fsc = make_double2(0.0, 0.0);
+    if constexpr (DET) {
+        gx_img = gsum + (long long)b * Hs * Ws * C;
+        fsc = fx_scale(fx_exp[b]);
+    }
 
     const uint32_t sb = smem_u32(smem), g_base = sb, w_base = sb + PC_GBYTES, f_base = w_base + 2 * PC_ABYTES;
     const int nch = C / PC_CK, kk2 = k * k, steps = kk2 * nch;
@@ -304,10 +315,16 @@ k_patch_conv_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                 }
 #pragma unroll
                 for (int c = 0; c < 4; ++c) {
-                    float* d = gs_img + (long long)q.o[c] * C + c0 + j * 8;
                     const float w = q.w[c];
-                    red_add_f32x4(d, w * a[0], w * a[1], w * a[2], w * a[3]);
-                    red_add_f32x4(d + 4, w * a[4], w * a[5], w * a[6], w * a[7]);
+                    if constexpr (DET) {
+                        fx_t* d = gx_img + (long long)q.o[c] * C + c0 + j * 8;
+#pragma unroll
+                        for (int e = 0; e < 8; ++e) fx_add(d + e, w * a[e], fsc);
+                    } else {
+                        float* d = gs_img + (long long)q.o[c] * C + c0 + j * 8;
+                        red_add_f32x4(d, w * a[0], w * a[1], w * a[2], w * a[3]);
+                        red_add_f32x4(d + 4, w * a[4], w * a[5], w * a[6], w * a[7]);
+                    }
                 }
             }
         }
@@ -326,10 +343,12 @@ k_patch_conv_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
 // ------------------------------------------------------------------------------------------- backward: weight gradient
 // CTA (blockIdx.x = tap t * nch + chunk, blockIdx.y = slice of pixel groups): grad_W[128 n][64 ch] += G^T A over its groups.
 // Warp w computes rows n 32 (w & 3) .. +32 and channels 32 (w >> 2) .. +32; both operands come through ldmatrix.trans.
+// DET: the slice sums go into the fixed-point sums gsum with the call's exponent fx_exp[0] (det_accum.cuh).
+template <bool DET = false>
 __global__ void __launch_bounds__(PC_THREADS, 2)
 k_patch_conv_wgrad_tc(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow, const __nv_bfloat16* __restrict__ gout,
                       float* __restrict__ gw, int C, int Hs, int Ws, int H, int W, int k, int gcols, int grows, int ngroups,
-                      int per_slice) {
+                      int per_slice, fx_t* __restrict__ gsum, const int* __restrict__ fx_exp) {
     extern __shared__ __align__(16) unsigned char smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
     const int wm = warp & 3, wn = warp >> 2;
@@ -413,7 +432,14 @@ k_patch_conv_wgrad_tc(const __nv_bfloat16* __restrict__ src, const float* __rest
         const int idx = i * PC_THREADS + tid, n = idx >> 4, j = idx & 15;
         float v[4];
         lds128f(f_base + n * PC_FSTR + j * 16, v);
-        red_add_f32x4(gw + ((long long)n * kk2 + t) * C + c0 + j * 4, v[0], v[1], v[2], v[3]);
+        if constexpr (DET) {
+            const double2 fsc = fx_scale(fx_exp[0]);
+            fx_t* d = gsum + ((long long)n * kk2 + t) * C + c0 + j * 4;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) fx_add(d + e, v[e], fsc);
+        } else {
+            red_add_f32x4(gw + ((long long)n * kk2 + t) * C + c0 + j * 4, v[0], v[1], v[2], v[3]);
+        }
     }
 }
 
@@ -442,6 +468,35 @@ int patch_conv_fwd(const void* src, const void* flow, const void* weight, void* 
     return launch_status();
 }
 
+template <bool DET>
+static int launch_patch_conv_bwd(const void* src, const void* flow, const void* weight, const void* gout, void* gsrc, void* gflow,
+                                 void* gweight, int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate, fx_t* gfx_src,
+                                 fx_t* gfx_w, const int* fx_exp, cudaStream_t st_) {
+    using namespace tc;
+    const int gcols = (W + GW - 1) / GW, grows = (H + GH - 1) / GH;
+    const long long ngroups = (long long)B * gcols * grows;
+    int r = set_smem((const void*)k_patch_conv_bwd_tc<DET>, PCB_SMEM);
+    if (r == GFLA_OK) r = set_smem((const void*)k_patch_conv_wgrad_tc<DET>, PCW_SMEM);
+    if (r != GFLA_OK) return r;
+    k_patch_conv_bwd_tc<DET><<<(unsigned)ngroups, PC_THREADS, PCB_SMEM, st_>>>((const __nv_bfloat16*)src, (const float*)flow,
+                                                                             (const __nv_bfloat16*)weight, (const __nv_bfloat16*)gout,
+                                                                             (float*)gsrc, (float*)gflow, C, Hs, Ws, H, W, k, gcols,
+                                                                             grows, accumulate, gfx_src, fx_exp);
+    r = launch_status();
+    if (r != GFLA_OK) return r;
+    // weight gradient: (tap, chunk) pairs x slices of pixel groups, about four CTAs per SM in all.  DET: slices of a fixed
+    // PCW_DET_GROUPS groups, so that the fp32 sums that become fixed-point partials depend on the shape only, not on the
+    // SM count
+    const int pairs = k * k * (C / PC_CK);
+    const long long want = (4LL * sm_count() + pairs - 1) / pairs;
+    const int per_slice = DET ? (int)min((long long)PCW_DET_GROUPS, ngroups) : (int)((ngroups + want - 1) / want);
+    const int slices = (int)((ngroups + per_slice - 1) / per_slice);
+    k_patch_conv_wgrad_tc<DET><<<dim3((unsigned)pairs, (unsigned)slices), PC_THREADS, PCW_SMEM, st_>>>(
+        (const __nv_bfloat16*)src, (const float*)flow, (const __nv_bfloat16*)gout, (float*)gweight, C, Hs, Ws, H, W, k, gcols, grows,
+        (int)ngroups, per_slice, gfx_w, DET ? fx_exp + B : nullptr);
+    return launch_status();
+}
+
 // accumulate = 0: the fp32 grad_source and grad_weight buffers are zero-filled here and grad_flow is overwritten; 1: all
 // three gradients are added into the caller's buffers
 int patch_conv_bwd(const void* src, const void* flow, const void* weight, const void* gout, void* gsrc, void* gflow, void* gweight,
@@ -455,24 +510,19 @@ int patch_conv_bwd(const void* src, const void* flow, const void* weight, const 
         if (z == GFLA_OK) z = zero_async(gweight, (size_t)PC_N * k * k * C * sizeof(float), st_);
         if (z != GFLA_OK) return z;
     }
-    int r = set_smem((const void*)k_patch_conv_bwd_tc, PCB_SMEM);
-    if (r == GFLA_OK) r = set_smem((const void*)k_patch_conv_wgrad_tc, PCW_SMEM);
-    if (r != GFLA_OK) return r;
-    k_patch_conv_bwd_tc<<<(unsigned)ngroups, PC_THREADS, PCB_SMEM, st_>>>((const __nv_bfloat16*)src, (const float*)flow,
-                                                                        (const __nv_bfloat16*)weight, (const __nv_bfloat16*)gout,
-                                                                        (float*)gsrc, (float*)gflow, C, Hs, Ws, H, W, k, gcols,
-                                                                        grows, accumulate);
-    r = launch_status();
-    if (r != GFLA_OK) return r;
-    // weight gradient: (tap, chunk) pairs x slices of pixel groups, about four CTAs per SM in all
-    const int pairs = k * k * (C / PC_CK);
-    const long long want = (4LL * sm_count() + pairs - 1) / pairs;
-    const int per_slice = (int)((ngroups + want - 1) / want);
-    const int slices = (int)((ngroups + per_slice - 1) / per_slice);
-    k_patch_conv_wgrad_tc<<<dim3((unsigned)pairs, (unsigned)slices), PC_THREADS, PCW_SMEM, st_>>>(
-        (const __nv_bfloat16*)src, (const float*)flow, (const __nv_bfloat16*)gout, (float*)gweight, C, Hs, Ws, H, W, k, gcols, grows,
-        (int)ngroups, per_slice);
-    return launch_status();
+    return launch_patch_conv_bwd<false>(src, flow, weight, gout, gsrc, gflow, gweight, B, C, Hs, Ws, H, W, k, accumulate, nullptr,
+                                        nullptr, nullptr, st_);
+}
+
+// grad_source and grad_weight into the fixed-point sums gsum_src / gfx_w (zeroed; exponents fx_exp[0, B) per image for
+// grad_source, fx_exp[B] for grad_weight: det_accum.cuh); grad_flow follows `accumulate`
+int patch_conv_bwd_det(const void* src, const void* flow, const void* weight, const void* gout, void* gflow, int B, int C, int Hs,
+                       int Ws, int H, int W, int k, int accumulate, fx_t* gfx_src, fx_t* gfx_w, const int* fx_exp, cudaStream_t st_) {
+    using namespace tc;
+    const long long ngroups = (long long)B * ((W + GW - 1) / GW) * ((H + GH - 1) / GH);
+    if (ngroups > INT_MAX) return GFLA_E_SHAPE;
+    return launch_patch_conv_bwd<true>(src, flow, weight, gout, nullptr, gflow, nullptr, B, C, Hs, Ws, H, W, k, accumulate, gfx_src,
+                                       gfx_w, fx_exp, st_);
 }
 
 }  // namespace gfla

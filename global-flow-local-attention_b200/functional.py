@@ -6,8 +6,17 @@ resample2d.py:10-11; `df == 2`: block_extractor.py:16; `ds == k*k`:
 local_attn_reshape.py:13; CPU tensors -> NotImplementedError:
 block_extractor.py:23-24, local_attn_reshape.py:20-21) and then hands raw
 device pointers to libgfla_warp.so on the caller's current stream.
+
+Under torch.use_deterministic_algorithms(True), read when a backward runs, the backward passes that scatter a gradient
+(local attention, block_extractor, patch convolution) run their deterministic variants (the *_det entry points: 64-bit
+fixed-point sums, bit-identical from run to run and independent of the batch composition); the resample2d backward,
+which has none, raises (warns with warn_only=True) like PyTorch's own ops.
 """
 from __future__ import annotations
+
+import contextlib
+import threading
+import warnings
 
 import torch
 
@@ -43,6 +52,50 @@ def _p(t):
     return None if t is None else t.data_ptr()
 
 
+# --------------------------------------------------------------------------- deterministic mode
+def alert_not_deterministic(caller: str) -> None:
+    """What PyTorch's ops do without a deterministic implementation: raise under torch.use_deterministic_algorithms(True),
+    warn instead with warn_only=True, nothing otherwise."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return
+    msg = (f"{caller} does not have a deterministic implementation, but you set 'torch.use_deterministic_algorithms(True)'. "
+           "You can turn off determinism just for this operation, or you can use the 'warn_only=True' option, if that's "
+           "acceptable for your application.")
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg, UserWarning, stacklevel=3)
+    else:
+        raise RuntimeError(msg)
+
+
+_FILL_LOCK = threading.Lock()
+
+
+@contextlib.contextmanager
+def _no_fill():
+    """In deterministic mode torch.empty fills new memory with NaN (torch.utils.deterministic.fill_uninitialized_memory).
+    What is allocated inside is written in full by the library (outputs), or zero-filled by the call that uses it
+    (workspaces), so that fill would only cost a pass over memory.  The setting is process-wide and autograd runs
+    backward passes on one thread per device: the lock keeps two of these blocks from interleaving, so each restores
+    the value it found."""
+    ud = torch.utils.deterministic
+    with _FILL_LOCK:
+        prev = ud.fill_uninitialized_memory
+        ud.fill_uninitialized_memory = False
+        try:
+            yield
+        finally:
+            ud.fill_uninitialized_memory = prev
+
+
+def _workspace(nbytes: int, device) -> torch.Tensor:
+    """caller-owned workspace of a *_det entry point (torch's caching allocator: 512-byte aligned, and it shows up in
+    torch.cuda's memory statistics)"""
+    if nbytes < 0:
+        raise _lib.GflaError(f"workspace query failed with code {nbytes}: {_lib.lib().gfla_error_string(nbytes).decode()}")
+    with _no_fill():
+        return torch.empty(nbytes, dtype=torch.uint8, device=device)
+
+
 # --------------------------------------------------------------------------- block_extractor
 def block_extract_fwd(source: torch.Tensor, flow: torch.Tensor, k: int) -> torch.Tensor:
     assert source.is_contiguous() and flow.is_contiguous()
@@ -72,6 +125,8 @@ def block_extract_bwd(source, flow, grad_out, k, grad_source=None, grad_flow=Non
     assert source.is_contiguous() and flow.is_contiguous()
     grad_out = grad_out.contiguous()
     _need_cuda(source, flow, grad_out)
+    if torch.are_deterministic_algorithms_enabled():
+        return _block_extract_bwd_det(source, flow, grad_out, k, grad_source, grad_flow)
     bs, ds, hs, ws = source.size()
     _, _, hf, wf = flow.size()
     accumulate, narrow, flow_in = 1, False, flow
@@ -95,6 +150,30 @@ def block_extract_bwd(source, flow, grad_out, k, grad_source=None, grad_flow=Non
         grad_source = convert(grad_source, source.dtype)
     if flow_in is not flow:
         grad_flow = convert(grad_flow, flow.dtype)
+    return grad_source, grad_flow
+
+
+def _block_extract_bwd_det(source, flow, grad_out, k, grad_source, grad_flow):
+    """grad_source summed in fixed point and rounded once to the source dtype (no fp32 buffer to narrow); grad_flow in one
+    channel slice, written once per element in the flow's dtype (no fp32 copy of a 16-bit flow needed)"""
+    bs, ds, hs, ws = source.size()
+    _, _, hf, wf = flow.size()
+    accumulate = 1
+    if grad_source is None:
+        accumulate = 0
+        with _no_fill():
+            grad_source, grad_flow = torch.empty_like(source), torch.empty_like(flow)
+    elif grad_source.dtype != source.dtype or grad_flow.dtype != flow.dtype:
+        # the sums are rounded once, into the source's (flow's) dtype: a wider buffer would only add a second rounding
+        raise TypeError(f"deterministic block_extract backward: grad_source / grad_flow must have the dtypes of source / "
+                        f"flow ({source.dtype} / {flow.dtype}), got {grad_source.dtype} / {grad_flow.dtype}")
+    l = _lib.lib()
+    nb = l.gfla_block_extract_bwd_det_workspace_bytes(bs, ds, hs, ws, hf, wf, k)
+    wsp = _workspace(nb, source.device)
+    with torch.cuda.device_of(source):
+        _lib.check(l.gfla_block_extract_bwd_det(_p(source), _p(flow), _p(grad_out), _p(grad_source), _p(grad_flow), bs, ds, hs, ws,
+                                                hf, wf, k, _dt(source), _dt(flow), accumulate, _p(wsp), nb, _stream(source)),
+                   "block_extract_bwd_det")
     return grad_source, grad_flow
 
 
@@ -142,6 +221,7 @@ def resample2d_fwd(input1: torch.Tensor, input2: torch.Tensor, kernel_size: int,
 
 
 def resample2d_bwd(input1, input2, grad_out, kernel_size, dilation, grad_input1=None, grad_input2=None):
+    alert_not_deterministic("resample2d backward (grad_input1 scatter)")
     assert input1.is_contiguous() and input2.is_contiguous()
     grad_out = grad_out.contiguous()
     _need_cuda(input1, input2, grad_out)
@@ -180,6 +260,8 @@ def resample2d_cosine_fwd(input1, input2, target, kernel_size: int, dilation: in
 def resample2d_cosine_bwd(input1, input2, target, stats, grad_cos, kernel_size, dilation, eps=1e-8, need_input1=False,
                           need_target=False):
     """-> (grad_input1 | None, grad_input2, grad_target | None)"""
+    if need_input1:
+        alert_not_deterministic("resample2d_cosine backward (grad_input1 scatter)")
     grad_cos = grad_cos.contiguous()
     _need_cuda(input1, input2, target, stats, grad_cos)
     _, d, hi, wi = input1.size()
@@ -320,6 +402,22 @@ def patch_conv_bwd(source, flow, weight, grad_out, k):
     _, _, h, w = flow.size()
     n = weight.shape[0]
     wp = _pack_weight(weight)
+    if torch.are_deterministic_algorithms_enabled():
+        # grad_source and grad_weight summed in fixed point and rounded once to bf16 by the library
+        with _no_fill():
+            gs = torch.empty((bs, hs, ws, ds), dtype=source.dtype, device=source.device)   # channels-last storage
+            gw = torch.empty((n, k, k, ds), dtype=weight.dtype, device=source.device)
+            gf = torch.empty_like(flow)
+        l = _lib.lib()
+        nb = l.gfla_patch_conv_bwd_det_workspace_bytes(bs, ds, hs, ws, h, w, k, n)
+        wsp = _workspace(nb, source.device)
+        with torch.cuda.device_of(source):
+            _lib.check(l.gfla_patch_conv_bwd_det(_p(src), _p(flow), _p(wp), _p(go), _p(gs), _p(gf), _p(gw), bs, ds, hs, ws, h, w, k, n,
+                                                 _dt(source), _dt(flow), _lib.GFLA_NHWC, 0, _p(wsp), nb, _stream(source)),
+                       "patch_conv_bwd_det")
+        del wsp
+        gs, gw = gs.permute(0, 3, 1, 2), gw.permute(0, 3, 1, 2)
+        return (relayout(gs, False) if planar else gs), gf, gw
     gs32 = torch.empty((bs, hs, ws, ds), dtype=torch.float32, device=source.device)   # channels-last storage
     gw32 = torch.empty((n, k, k, ds), dtype=torch.float32, device=source.device)
     gf = torch.empty_like(flow)
@@ -354,6 +452,8 @@ def local_attn_bwd(source, flow, logits, grad_out, k, algo="auto"):
         return relayout(gs, False), gf, gl
     fmt = torch.channels_last if layout == _lib.GFLA_NHWC else torch.contiguous_format
     grad_out = grad_out.contiguous(memory_format=fmt)
+    if torch.are_deterministic_algorithms_enabled():
+        return _local_attn_bwd_det(source, flow, logits, grad_out, k, layout, algo)
     tile = layout == _lib.GFLA_NHWC and _tile_bwd_eligible(source, flow, k)
     if source.dtype in (torch.bfloat16, torch.float16) and (algo == "gather" or (algo == "auto" and not tile)):
         # The CUDA-core backward scatters grad_source with one atomic add per (pixel, tap, channel).  In a 16-bit type every
@@ -368,4 +468,21 @@ def local_attn_bwd(source, flow, logits, grad_out, k, algo="auto"):
         _lib.check(_lib.lib().gfla_local_attn_bwd(_p(source), _p(flow), _p(logits), _p(grad_out), _p(gs), _p(gf), _p(gl),
                                                   bs, ds, hs, ws, h, w, k, _dt(source), _dt(flow), layout, 0, ALGO[algo],
                                                   _stream(source)), "local_attn_bwd")
+    return gs, gf, gl
+
+
+def _local_attn_bwd_det(source, flow, logits, grad_out, k, layout, algo):
+    """grad_source summed in fixed point and rounded once to the source dtype, by the tile or the gather kernel: 16-bit
+    gather calls need no fp32 copies here"""
+    bs, ds, hs, ws = source.size()
+    _, _, h, w = flow.size()
+    with _no_fill():
+        gs, gf, gl = _like_layout(source, source.shape, layout), torch.empty_like(flow), torch.empty_like(logits)
+    l = _lib.lib()
+    nb = l.gfla_local_attn_bwd_det_workspace_bytes(bs, ds, hs, ws, h, w, k)
+    wsp = _workspace(nb, source.device)
+    with torch.cuda.device_of(source):
+        _lib.check(l.gfla_local_attn_bwd_det(_p(source), _p(flow), _p(logits), _p(grad_out), _p(gs), _p(gf), _p(gl), bs, ds, hs, ws, h,
+                                             w, k, _dt(source), _dt(flow), layout, 0, ALGO[algo], _p(wsp), nb, _stream(source)),
+                   "local_attn_bwd_det")
     return gs, gf, gl

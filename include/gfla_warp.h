@@ -244,6 +244,46 @@ int gfla_patch_conv_bwd(const void* source, const void* flow, const void* weight
                         int B, int C, int Hs, int Ws, int H, int W, int k, int N,
                         int dtype, int flow_dtype, int layout, int accumulate, gfla_stream_t stream);
 
+/* ------------------------------------------------------------------------ *
+ * deterministic backward passes  (torch.use_deterministic_algorithms(True))
+ *   The same gradients as gfla_local_attn_bwd, gfla_block_extract_bwd and gfla_patch_conv_bwd, bit-identical from call
+ *   to call and independent of the batch composition: each scattered gradient (grad_source, and grad_weight of the
+ *   patch convolution) is summed as 64-bit fixed point with one power-of-two scale per image (per call for
+ *   grad_weight) derived on the device from max|grad_out| and a proved bound, then rounded once to `dtype`.
+ *   The other gradients (grad_flow, grad_logits) are written per pixel as in the default entry points.
+ *   - workspace: caller-owned DEVICE memory of at least *_det_workspace_bytes(...) bytes, 16-byte aligned; its
+ *     contents on entry do not matter (the call zero-fills what it uses).  NULL: GFLA_E_NULL; misaligned:
+ *     GFLA_E_ALIGN; too small: GFLA_E_SHAPE (nothing is launched in each case).  The *_workspace_bytes queries
+ *     return a negative GFLA_E_* code for bad sizes.
+ *   - a non-finite value among the inputs of an image's bound (grad_out; for the patch convolution also the weight and,
+ *     for grad_weight, the source) makes every fixed-point output of that image (of the call, for grad_weight) NaN.
+ *   - an image whose grad_out is all zero gets exactly zero (plus the caller's value with accumulate = 1).
+ *   - a partial that is non-finite for another reason (NaN or Inf logits, flow or source) is not made sticky: it
+ *     converts to INT64_MIN and the sums it lands in are meaningless (not necessarily NaN).
+ *   - the results do not depend on the SM count: no launch shape of these entry points follows it.
+ *   gfla_block_extract_bwd_det: grad_source has the data dtype (no fp32 variant: the sum is rounded once anyway).
+ *   gfla_patch_conv_bwd_det: grad_source [B,Hs,Ws,C] and grad_weight [N][k][k][C] in `dtype` (channels-last storage).
+ * ------------------------------------------------------------------------ */
+long long gfla_local_attn_bwd_det_workspace_bytes(int B, int C, int Hs, int Ws, int H, int W, int k);
+int gfla_local_attn_bwd_det(const void* source, const void* flow, const void* logits,
+                            const void* grad_out,
+                            void* grad_source, void* grad_flow, void* grad_logits,
+                            int B, int C, int Hs, int Ws, int H, int W, int k,
+                            int dtype, int flow_dtype, int layout, int accumulate, int algo,
+                            void* workspace, long long workspace_bytes, gfla_stream_t stream);
+long long gfla_block_extract_bwd_det_workspace_bytes(int B, int C, int Hs, int Ws, int Hf, int Wf, int k);
+int gfla_block_extract_bwd_det(const void* source, const void* flow, const void* grad_out,
+                               void* grad_source, void* grad_flow,
+                               int B, int C, int Hs, int Ws, int Hf, int Wf, int k,
+                               int dtype, int flow_dtype, int accumulate,
+                               void* workspace, long long workspace_bytes, gfla_stream_t stream);
+long long gfla_patch_conv_bwd_det_workspace_bytes(int B, int C, int Hs, int Ws, int H, int W, int k, int N);
+int gfla_patch_conv_bwd_det(const void* source, const void* flow, const void* weight, const void* grad_out,
+                            void* grad_source, void* grad_flow, void* grad_weight,
+                            int B, int C, int Hs, int Ws, int H, int W, int k, int N,
+                            int dtype, int flow_dtype, int layout, int accumulate,
+                            void* workspace, long long workspace_bytes, gfla_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

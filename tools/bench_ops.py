@@ -107,6 +107,95 @@ if "patch_conv" in which:   # ExtractorAttn's source-half conv: materialised (Bl
         del src, flow, w, g
         torch.cuda.empty_cache()
 
+if "det" in which:   # torch.use_deterministic_algorithms(True) against the default mode, alternated in one process
+    import statistics
+    import subprocess
+    from torch.profiler import ProfilerActivity, profile
+    from gfla_b200.extractor_attn import PatchConvFunction
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+    card = q.stdout.strip() or torch.cuda.get_device_name(0)
+    cl = torch.channels_last
+    B, C, HW, k = 16, 256, 256, 5          # cfg2
+    src = torch.randn(B, C, HW, HW, device=dev).bfloat16().contiguous(memory_format=cl)
+    flow = smooth(B, HW, HW)
+    logits = torch.randn(B, k * k, HW, HW, device=dev).bfloat16()
+    gout = torch.randn(B, C, HW, HW, device=dev).bfloat16().contiguous(memory_format=cl)
+
+    def step():
+        F_.local_attn_fwd(src, flow, logits, k)
+        F_.local_attn_bwd(src, flow, logits, gout, k)
+
+    def bwd():
+        F_.local_attn_bwd(src, flow, logits, gout, k)
+
+    def in_mode(det, fn):
+        torch.use_deterministic_algorithms(det)
+        try:
+            return fn()
+        finally:
+            torch.use_deterministic_algorithms(False)
+
+    res = {False: {"step": [], "bwd": []}, True: {"step": [], "bwd": []}}
+    for _ in range(5):
+        for det in (False, True):
+            res[det]["step"].append(in_mode(det, lambda: timed(step, n=5, w=2)))
+            res[det]["bwd"].append(in_mode(det, lambda: timed(bwd, n=5, w=2)))
+    peak = {}
+    for det in (False, True):
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        base = torch.cuda.memory_allocated()
+        in_mode(det, step)
+        torch.cuda.synchronize()
+        peak[det] = round((torch.cuda.max_memory_allocated() - base) / 2 ** 20, 1)
+
+    def breakdown(det):
+        in_mode(det, bwd)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            in_mode(det, bwd)
+            torch.cuda.synchronize()
+        parts = {"pre-pass (k_fx_amax, k_fx_exponents)": 0.0, "memset": 0.0, "backward kernel": 0.0, "k_fold_border": 0.0,
+                 "narrowing (k_fx_narrow)": 0.0, "other": 0.0}
+        for e in prof.key_averages():
+            us = getattr(e, "device_time_total", 0.0) or getattr(e, "cuda_time_total", 0.0)
+            n = e.key
+            key = ("pre-pass (k_fx_amax, k_fx_exponents)" if ("k_fx_amax" in n or "k_fx_exponents" in n) else
+                   "memset" if "emset" in n else "backward kernel" if "k_local_attn_bwd" in n else
+                   "k_fold_border" if "k_fold_border" in n else "narrowing (k_fx_narrow)" if "k_fx_narrow" in n else "other")
+            parts[key] += us / 1e3
+        return {a: round(b, 4) for a, b in parts.items()}
+
+    med = lambda v: round(statistics.median(v), 4)
+    print(json.dumps({"op": "local attention fwd+bwd, default vs deterministic mode",
+                      "config": f"cfg2: B={B} C={C} {HW}x{HW} k={k} bf16 channels_last, smooth flow",
+                      "step_ms": {"default": med(res[False]["step"]), "deterministic": med(res[True]["step"])},
+                      "bwd_ms": {"default": med(res[False]["bwd"]), "deterministic": med(res[True]["bwd"])},
+                      "step_ms_all": {"default": [round(v, 4) for v in res[False]["step"]],
+                                      "deterministic": [round(v, 4) for v in res[True]["step"]]},
+                      "bwd_breakdown_ms": {"default": breakdown(False), "deterministic": breakdown(True)},
+                      "peak_MB_above_inputs_step": {"default": peak[False], "deterministic": peak[True]},
+                      "card_and_power_limit": card,
+                      "timing": "CUDA events, median of 5 alternating rounds of 5 calls; breakdown from one profiled call"}),
+          flush=True)
+    del src, flow, logits, gout
+    torch.cuda.empty_cache()
+    for (Bp, Cp, HWp, kp) in ((8, 256, 32, 3), (8, 128, 64, 5), (2, 256, 256, 5)):
+        s_ = torch.randn(Bp, Cp, HWp, HWp, device=dev).bfloat16().contiguous(memory_format=cl).requires_grad_()
+        f_ = (torch.rand(Bp, 2, HWp, HWp, device=dev) * 8 - 4).requires_grad_()
+        w_ = (torch.randn(128, Cp, kp, kp, device=dev) / (Cp * kp * kp) ** 0.5).bfloat16().requires_grad_()
+        g_ = torch.randn(Bp, 128, HWp, HWp, device=dev).bfloat16().contiguous(memory_format=cl)
+        fb = lambda: PatchConvFunction.apply(s_, f_, w_, kp).backward(g_)
+        pr = {False: [], True: []}
+        for _ in range(5):
+            for det in (False, True):
+                pr[det].append(in_mode(det, lambda: timed(fb, n=3, w=1)))
+        print(json.dumps({"op": "patch conv fwd+bwd, default vs deterministic mode",
+                          "config": f"B={Bp} C={Cp} {HWp}x{HWp} k={kp} N=128 bf16 channels_last",
+                          "fwd_bwd_ms": {"default": med(pr[False]), "deterministic": med(pr[True])},
+                          "card_and_power_limit": card, "timing": "CUDA events, median of 5 alternating rounds"}), flush=True)
+        del s_, f_, w_, g_
+        torch.cuda.empty_cache()
+
 if "module" in which:   # ExtractorAttn at the shapes the pose generator uses (SURVEY.md section 3): fused module vs the literal op chain
     import gfla_b200
     for (C, HW, k) in ((256, 32, 3), (128, 64, 5)):
