@@ -2,13 +2,15 @@
 //
 // Per 16x8 pixel group the weighted gather is a dense GEMM
 //     out[128 px][C] = Wfull[128 px][footprint] * S[footprint][C]
-// with K running over the source positions of the group's tap footprint, one row segment of 16 positions per step:
+// with K running over the source positions of the group's tap footprint, one row segment per step (32 positions = two MMA
+// K-steps for channels-last, 16 for planar; FwdGeom):
 //   * one thread per pixel: softmax, taps (exactly like block_extractor_kernel.cu:62-76), the collapsed (k+1)^2 window
 //     (tile_window.cuh) kept in registers;
-//   * per step every thread writes its pixel's row of the weight slab A[128 px][16 pos] (bf16; at most k+1 non-zeros),
-//     the source segment B[16 pos][64 ch] arrives by cp.async (channels-last) or plain loads (planar) one step ahead;
-//   * warp w multiplies pixel rows 32w..32w+31 with mma.sync m16n8k16 (fp32 accumulators in registers), skipping the
-//     16-pixel m-tiles none of whose windows meets the step (window_meets_step: their slab rows are all zero);
+//   * per step every thread writes its pixel's row of the weight slab A[128 px][NPOS] (bf16; at most k+1 non-zeros),
+//     the source segment B[NPOS][64 ch] arrives by cp.async through a ring FT_STAGES - 1 steps ahead, across channel
+//     passes (channels-last), or by plain loads one step ahead (planar);
+//   * warp w multiplies pixel rows 32w..32w+31 with mma.sync m16n8k16 (fp32 accumulators in registers), skipping per
+//     K-step the 16-pixel m-tiles none of whose windows meets it (window_meets_step: their slab rows are all zero);
 //   * pixels whose taps are not consecutive integers keep the literal 4-tap arithmetic (irregular_pixel, warp-cooperative).
 #include "tile_window.cuh"
 
@@ -17,60 +19,83 @@ namespace tc {
 
 constexpr int FT_THREADS = 128;                 // one thread per pixel of the group
 constexpr int FT_CN = 64;                       // channels per pass (N of the MMAs)
-constexpr int FT_ASTR = SEG * 2 + 16;           // weight-slab row: 32 B + 16 B pad (conflict-free ldmatrix)
 constexpr int FT_BSTR = FT_CN * 2 + 16;         // source-segment row: 128 B + 16 B pad
+constexpr int FT_STAGES = 4;                    // channels-last source-segment ring: FT_STAGES - 1 segments ahead (DESIGN 3.2)
 
+// Source positions per step: channels-last walks the footprint in segments of two MMA K-steps (2 x SEG), which halves the
+// steps, barriers and per-step bookkeeping; planar keeps SEG (its next segment is staged in registers).
+template <bool NHWC>
+struct FwdGeom {
+    static constexpr int NPOS = NHWC ? 2 * SEG : SEG;
+    static constexpr int HALVES = NPOS / SEG;               // MMA K-steps per step
+    static constexpr int ASTR = NPOS * 2 + 16;              // weight-slab row: NPOS bf16 + 16 B pad (conflict-free ldmatrix)
+    static constexpr int BSEG = NPOS * FT_BSTR;             // one source segment in shared memory
+    static constexpr int NBUF = NHWC ? FT_STAGES : 2;       // source-segment buffers
+};
+
+template <bool NHWC>
 struct FwdSmem {
-    alignas(16) unsigned char a[2][128 * FT_ASTR];
-    alignas(16) unsigned char b[2][SEG * FT_BSTR];
+    alignas(16) unsigned char a[2][128 * FwdGeom<NHWC>::ASTR];
+    alignas(16) unsigned char b[FwdGeom<NHWC>::NBUF][FwdGeom<NHWC>::BSEG];
     int irr[128];
     int nirr;
 };
 
-template <bool NHWC>
-struct SegLoad {
-    __nv_bfloat16 v[NHWC ? 1 : 8];
+// planar: source row segment (16 positions from x, clamped at the right edge: those columns carry zero weight) x 64
+// channels, loaded into registers one step ahead and stored to shared memory after the step's MMAs
+struct SegRegs {
+    __nv_bfloat16 v[8];
 };
-
-// source row segment (16 positions from x, clamped at the right edge: those columns carry zero weight) x 64 channels
-template <bool NHWC>
-__device__ __forceinline__ void seg_issue(const __nv_bfloat16* __restrict__ src, int b, int C, int c0, int Hs, int Ws, int y, int x,
-                                          uint32_t dst, int tid, SegLoad<NHWC>& r) {
-    if constexpr (NHWC) {
-        const int i = tid >> 3, j = tid & 7;              // position, 8-channel chunk
-        const int xs = min(x + i, Ws - 1);
-        cp_async16(dst + i * FT_BSTR + j * 16, src + (((long long)b * Hs + y) * Ws + xs) * C + c0 + j * 8);
-        cp_async_commit();
-    } else {
+__device__ __forceinline__ void seg_load(const __nv_bfloat16* __restrict__ src, int b, int C, int c0, int Hs, int Ws, int y, int x,
+                                         int tid, SegRegs& r) {
 #pragma unroll
-        for (int it = 0; it < 8; ++it) {
-            const int idx = it * FT_THREADS + tid, c = idx >> 4, i = idx & 15;
-            const int xs = min(x + i, Ws - 1);
-            r.v[it] = src[(((long long)b * C + c0 + c) * Hs + y) * Ws + xs];
-        }
+    for (int it = 0; it < 8; ++it) {
+        const int idx = it * FT_THREADS + tid, c = idx >> 4, i = idx & 15;
+        const int xs = min(x + i, Ws - 1);
+        r.v[it] = src[(((long long)b * C + c0 + c) * Hs + y) * Ws + xs];
     }
 }
-template <bool NHWC>
-__device__ __forceinline__ void seg_store(uint32_t dst, int tid, const SegLoad<NHWC>& r) {
-    if constexpr (!NHWC) {
+__device__ __forceinline__ void seg_store(uint32_t dst, int tid, const SegRegs& r) {
 #pragma unroll
-        for (int it = 0; it < 8; ++it) {
-            const int idx = it * FT_THREADS + tid, c = idx >> 4, i = idx & 15;
-            sts16(dst + i * FT_BSTR + c * 2, static_cast<uint32_t>(*reinterpret_cast<const unsigned short*>(&r.v[it])));
+    for (int it = 0; it < 8; ++it) {
+        const int idx = it * FT_THREADS + tid, c = idx >> 4, i = idx & 15;
+        sts16(dst + i * FT_BSTR + c * 2, static_cast<uint32_t>(*reinterpret_cast<const unsigned short*>(&r.v[it])));
+    }
+}
+
+// channels-last: the producer of the segment ring.  Copies the segment at (c0, y, x) (NPOS positions, clamped at the right
+// edge like the planar segment) with cp.async, then moves (c0, y, x) on in the consumer's order: row-major over the
+// footprint, then on into the next 64-channel pass.  Past the last pass it copies nothing, but it commits a group on every
+// call, so that the consumer's wait count holds to the end.
+template <int NPOS>
+__device__ __forceinline__ void seg_produce(const __nv_bfloat16* __restrict__ src, int b, int C, int Hs, int Ws, int bx0, int by0,
+                                            int bx1, int by1, int& c0, int& y, int& x, uint32_t dst, int tid) {
+    if (c0 < C) {
+        const int j = tid & 7;                            // 8-channel chunk
+        const __nv_bfloat16* row = src + ((long long)b * Hs + y) * Ws * C + c0 + j * 8;
+#pragma unroll
+        for (int i = tid >> 3; i < NPOS; i += FT_THREADS / 8)   // position
+            cp_async16(dst + i * FT_BSTR + j * 16, row + (long long)min(x + i, Ws - 1) * C);
+        x += NPOS;
+        if (x > bx1) {
+            x = bx0;
+            if (++y > by1) { y = by0; c0 += FT_CN; }
         }
     }
+    cp_async_commit();
 }
 
 // Channels-last: at most 168 registers, so that three CTAs share an SM and hide each other's per-step barrier (cfg2 on an
 // H100 80GB HBM3 at 400 W: 1.67 ms against 2.21 ms at two CTAs).  The planar kernel holds its next source segment in
-// registers (SegLoad) and stays at two.
+// registers (SegRegs) and stays at two.
 template <int K, bool NHWC>
 __global__ void __launch_bounds__(FT_THREADS, NHWC ? 3 : 1)
 k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow, const __nv_bfloat16* __restrict__ logits,
                     __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ probs, const __nv_bfloat16* __restrict__ prev,
                     const __nv_bfloat16* __restrict__ mask, int C, int Hs, int Ws, int H, int W, int gcols, int grows) {
     constexpr int K1 = K + 1, KK = K * K;
-    __shared__ FwdSmem sm;
+    using G = FwdGeom<NHWC>;
+    __shared__ FwdSmem<NHWC> sm;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
     uint32_t b;
     int gx0, gy0;
@@ -78,6 +103,17 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     const long long hw = (long long)H * W;
 
     if (tid == 0) sm.nirr = 0;
+    int bx0, by0, bx1, by1;
+    group_bbox<K>(flow, b, gx0, gy0, H, W, Hs, Ws, lane, bx0, by0, bx1, by1);
+    const uint32_t a_base = smem_u32(sm.a[0]), b_base = smem_u32(sm.b[0]);
+    // channels-last: the producer (nc0, ny, nx) runs FT_STAGES - 1 segments ahead of the steps; the first ones load while
+    // the pixels compute their windows
+    int nc0 = 0, ny = by0, nx = bx0;
+    if constexpr (NHWC) {
+#pragma unroll
+        for (int s = 0; s < FT_STAGES - 1; ++s)
+            seg_produce<G::NPOS>(src, b, C, Hs, Ws, bx0, by0, bx1, by1, nc0, ny, nx, b_base + s * G::BSEG, tid);
+    }
     __syncthreads();
     // ---- per pixel: softmax, taps, window
     const int px = gx0 + (tid & 15), py = gy0 + (tid >> 4);
@@ -98,17 +134,16 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
         if (regular) build_window<K>(p, tx, ty, Hs, Ws, 1.0f / static_cast<float>(KK), w, X0, Y0);
         else sm.irr[atomicAdd(&sm.nirr, 1)] = tid;
     }
-    int bx0, by0, bx1, by1;
-    group_bbox<K>(flow, b, gx0, gy0, H, W, Hs, Ws, lane, bx0, by0, bx1, by1);
 
-    const uint32_t a_base = smem_u32(sm.a[0]), b_base = smem_u32(sm.b[0]);
-    const uint32_t a_row = a_base + tid * FT_ASTR;
+    const uint32_t a_row = a_base + tid * G::ASTR;
     // ldmatrix lane addresses: A (rows = pixels of this warp, K = positions), B (rows = positions, N = channels, transposed)
-    const uint32_t a_frag = a_base + (warp * 32 + (lane & 15)) * FT_ASTR + (lane >> 4) * 16;
+    const uint32_t a_frag = a_base + (warp * 32 + (lane & 15)) * G::ASTR + (lane >> 4) * 16;
     const uint32_t b_frag = b_base + (lane & 15) * FT_BSTR + (lane >> 4) * 16;
 
+    // Steps: channels-last numbers them t = 0, 1, ... across all passes (one flat stream), planar restarts at every pass.
+    // The weight slab alternates its two buffers with t; the channels-last step t reads ring slot t % FT_STAGES.
+    int t = 0, slot = 0;
     for (int c0 = 0; c0 < C; c0 += FT_CN) {
-        __syncthreads();          // the previous pass's MMAs are done with both buffers
         float acc[2][8][4];
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt)
@@ -116,47 +151,72 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
             for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
                 for (int q = 0; q < 4; ++q) acc[mt][nt][q] = 0.f;
-        SegLoad<NHWC> pend;
-        seg_issue<NHWC>(src, b, C, c0, Hs, Ws, by0, bx0, b_base, tid, pend);
-        seg_store<NHWC>(b_base, tid, pend);
-        // steps walk the footprint row-major: y from by0, x = bx0, bx0 + SEG, ... while x <= bx1
-        for (int s = 0, y = by0, x = bx0; y <= by1; ++s) {
-            const int buf = s & 1;
-            int xn = x + SEG, yn = y;
+        SegRegs pend;
+        if constexpr (!NHWC) {
+            __syncthreads();      // the previous pass's MMAs are done with both buffers
+            t = 0;
+            seg_load(src, b, C, c0, Hs, Ws, by0, bx0, tid, pend);
+            seg_store(b_base, tid, pend);
+        }
+        // steps walk the footprint row-major: y from by0, x = bx0, bx0 + NPOS, ... while x <= bx1
+        for (int y = by0, x = bx0; y <= by1; ++t) {
+            const int buf = t & 1;
+            int xn = x + G::NPOS, yn = y;
             if (xn > bx1) { xn = bx0; ++yn; }
             // this pixel's row of the weight slab: zeros except window row y - Y0
-            const uint32_t row = a_row + buf * (128 * FT_ASTR);
-            sts128(row, 0u, 0u, 0u, 0u);
-            sts128(row + 16, 0u, 0u, 0u, 0u);
-            const bool act = regular && window_meets_step<K>(X0, Y0, Hs, Ws, y, x);
-            if (act) scatter_window_row<K>(row, 2, w, X0, Y0, y, x);
-            // m-tiles (16 pixels each) of this warp with an active pixel: the others' slab rows are all zero
-            const uint32_t wm = warp_row_bits(act);
-            if (NHWC) cp_async_wait_all();
-            __syncthreads();      // slab and segment of step s complete; everybody is past step s-1's MMAs
-            const bool more = yn <= by1;
-            if (more) seg_issue<NHWC>(src, b, C, c0, Hs, Ws, yn, xn, b_base + (buf ^ 1) * (SEG * FT_BSTR), tid, pend);
-            if (wm != 0u) {
+            const uint32_t row = a_row + buf * (128 * G::ASTR);
+#pragma unroll
+            for (int q = 0; q < G::NPOS * 2; q += 16) sts128(row + q, 0u, 0u, 0u, 0u);
+            // per MMA K-step (SEG positions): the m-tiles (16 pixels each) of this warp with an active pixel; the others'
+            // slab rows are all zero there
+            uint32_t wm[G::HALVES];
+            bool act = false;
+#pragma unroll
+            for (int hk = 0; hk < G::HALVES; ++hk) {
+                const bool a = regular && window_meets_step<K>(X0, Y0, Hs, Ws, y, x + hk * SEG);
+                wm[hk] = warp_row_bits(a);
+                act |= a;
+            }
+            if (act) scatter_window_row<K, G::NPOS>(row, 2, w, X0, Y0, y, x);
+            uint32_t bseg;
+            if constexpr (NHWC) {
+                cp_async_wait<FT_STAGES - 2>();   // this thread's part of step t's segment has landed
+                __syncthreads();      // slab and segment of step t complete; everybody is past step t-1's MMAs
+                // so step t-1's slot is free: it takes the segment of step t + FT_STAGES - 1
+                const int free_slot = slot == 0 ? FT_STAGES - 1 : slot - 1;
+                seg_produce<G::NPOS>(src, b, C, Hs, Ws, bx0, by0, bx1, by1, nc0, ny, nx, b_base + free_slot * G::BSEG, tid);
+                bseg = slot * G::BSEG;
+                slot = slot == FT_STAGES - 1 ? 0 : slot + 1;
+            } else {
+                __syncthreads();      // slab and segment of step t complete; everybody is past step t-1's MMAs
+                if (yn <= by1) seg_load(src, b, C, c0, Hs, Ws, yn, xn, tid, pend);
+                bseg = buf * G::BSEG;
+            }
+            // K-steps in position order: every accumulator receives the same MMAs in the same order as with SEG-wide steps
+#pragma unroll
+            for (int hk = 0; hk < G::HALVES; ++hk) {
+                if (wm[hk] == 0u) continue;
+                const uint32_t a_k = a_frag + buf * (128 * G::ASTR) + hk * (SEG * 2);
                 uint32_t af[2][4];
-                if (wm & 1u) ldsm_x4(a_frag + buf * (128 * FT_ASTR), af[0]);
-                if (wm & 2u) ldsm_x4(a_frag + buf * (128 * FT_ASTR) + 16 * FT_ASTR, af[1]);
+                if (wm[hk] & 1u) ldsm_x4(a_k, af[0]);
+                if (wm[hk] & 2u) ldsm_x4(a_k + 16 * G::ASTR, af[1]);
 #pragma unroll
                 for (int np = 0; np < 4; ++np) {
                     uint32_t bf[4];
-                    ldsm_x4_t(b_frag + buf * (SEG * FT_BSTR) + np * 32, bf);
+                    ldsm_x4_t(b_frag + bseg + hk * (SEG * FT_BSTR) + np * 32, bf);
 #pragma unroll
                     for (int mt = 0; mt < 2; ++mt) {
-                        if (((wm >> mt) & 1u) == 0u) continue;
+                        if (((wm[hk] >> mt) & 1u) == 0u) continue;
                         mma_bf16(acc[mt][2 * np], af[mt], bf[0], bf[1]);
                         mma_bf16(acc[mt][2 * np + 1], af[mt], bf[2], bf[3]);
                     }
                 }
             }
-            if (more) seg_store<NHWC>(b_base + (buf ^ 1) * (SEG * FT_BSTR), tid, pend);
+            if (!NHWC && yn <= by1) seg_store(b_base + (buf ^ 1) * G::BSEG, tid, pend);
             x = xn;
             y = yn;
         }
-        // ---- epilogue: rows = pixels, columns = channels c0 + 8 nt + 2 tig (+1)
+        // ---- epilogue: rows = pixels, columns = channels c0 + 8 nt + 2 tig (+1); channels-last keeps loading meanwhile
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt)
 #pragma unroll

@@ -33,6 +33,9 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+// wait until at most N of this thread's committed groups are still in flight
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ------------------------------------------------------------------ ldmatrix / mma
 // four 8x8 b16 matrices; lane l supplies the row address of matrix l/8

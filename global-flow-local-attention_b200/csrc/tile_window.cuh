@@ -120,9 +120,9 @@ __device__ __forceinline__ void build_window(const float* p, const AxisTap<float
     for (int i = 0; i < K1 * K1 / 2; ++i) wp[i] = bf16_bits(w[2 * i]) | (bf16_bits(w[2 * i + 1]) << 16);
 }
 
-// This pixel's weights for source row y, positions [x, x + SEG): window row y - Y0 (nothing when the row is outside the
+// This pixel's weights for source row y, positions [x, x + NPOS): window row y - Y0 (nothing when the row is outside the
 // window), stored as bf16 at base + e * stride for position x + e.  The zero entries are the caller's to write.
-template <int K>
+template <int K, int NPOS = SEG>
 __device__ __forceinline__ void scatter_window_row(uint32_t base, uint32_t stride, const uint32_t (&wp)[(K + 1) * (K + 1) / 2],
                                                    int X0, int Y0, int y, int x) {
     constexpr int K1 = K + 1, RW = K1 / 2;   // bf16 pairs per window row
@@ -141,7 +141,7 @@ __device__ __forceinline__ void scatter_window_row(uint32_t base, uint32_t strid
     for (int s = 0; s < K1; ++s) {
         const int e = X0 + s - x;
         const uint32_t h = (s & 1) ? wr[s / 2] >> 16 : wr[s / 2] & 0xffffu;
-        if (e >= 0 && e < SEG && (h & 0x7fffu) != 0u) sts16(base + e * stride, h);
+        if (e >= 0 && e < NPOS && (h & 0x7fffu) != 0u) sts16(base + e * stride, h);
     }
 }
 
