@@ -253,13 +253,12 @@ __device__ __forceinline__ void rs_in2_store(const RsTaps<A, NT>& t, A sum, cons
             sgrad[2] += (rTL * wTL + rTR * wTR + rBL * wBL + rBR * wBR) / den_s;
             wd += wTL * d[0] + wTR * d[1] + wBL * d[2] + wBR * d[3];
         }
-    const double S = static_cast<double>(sum);
-    const double inv1 = (sum == static_cast<A>(0)) ? 1e8 : 1.0 / S;
-    const double S2 = static_cast<double>(sum * sum);
-    const double inv2 = (sum * sum == static_cast<A>(0)) ? 1e8 : 1.0 / S2;
+    // quotients, not reciprocals: in fp64 a subnormal sum*sum has no finite reciprocal, while g2 / (sum*sum) stays finite
+    const double S = (sum == static_cast<A>(0)) ? 1e-8 : static_cast<double>(sum);
+    const double S2 = (sum * sum == static_cast<A>(0)) ? 1e-8 : static_cast<double>(sum * sum);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-        const A v = static_cast<A>(g1[c] * inv1 - (sgrad[c] * wd) * inv2);
+        const A v = static_cast<A>(g1[c] / S - (sgrad[c] * wd) / S2);
         gp[c * opl] = accumulate ? gp[c * opl] + v : v;
     }
 }
