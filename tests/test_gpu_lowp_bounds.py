@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import ref64
+import ref64_gather
 from test_ref64 import make_flow
 
 pytestmark = pytest.mark.gpu
@@ -136,35 +137,36 @@ def test_tile_backward_bf16_accumulate(F_, kind, k):
               ref64.bound_gs_tile(r["Mgs"], r["n_adds"][:, None], u, eta, init=init[0]), init=init)
 
 
-@pytest.mark.parametrize("k", [1, 3, 4, 5])
+@pytest.mark.parametrize("k", range(1, 10))
 @pytest.mark.parametrize("flow_dt", ["fp32", "storage"])
 @pytest.mark.parametrize("dt", ["bf16", "fp16"])
 def test_gather_16bit(F_, dt, flow_dt, k):
-    """the CUDA-core kernels in 16-bit storage: fp32 arithmetic, one rounding per output (the backward runs on fp32
-    copies); with an fp32 flow and with a flow in the storage dtype"""
+    """the CUDA-core kernels in 16-bit storage: the fp32 kernels' arithmetic on the widened values (their ref64_gather
+    bound, which grows with k and C) and one rounding per output (the backward runs on fp32 copies); with an fp32 flow and
+    with a flow in the storage dtype"""
     B, C, Hs, Ws, H, W = 2, 48, 23, 29, 23, 29
     fdt = torch.float32 if flow_dt == "fp32" else TDT[dt]
     u, eta = ref64.storage(dt)
+    b = lambda y, e32: ref64.bound_gather16(y, e32, u, eta)
     for kind in ("smooth", "border", "irregular") if k > 1 else ("smooth", "border"):   # one tap: always regular
         s, f, lg, g = make(B, C, Hs, Ws, H, W, k, kind, seed=7 * k + len(kind) + len(dt), dt=dt, flow_dt=fdt)
-        la = ref64.LocalAttn(host(f), host(lg), k, Hs, Ws)
-        r, M = la.fwd(host(s))
+        la = ref64_gather.LocalAttn(host(f), host(lg), k, Hs, Ws, np.float32)
+        r, mags = la.fwd(host(s))
         out, probs = F_.local_attn_fwd(s, f, lg, k, return_probs=True, algo="gather")
-        within(f"out gather {dt}", out, r, ref64.bound_out_gather(r, M, u, eta), M=M)
-        within(f"probs gather {dt}", probs, la.probs(), ref64.bound_probs(la.probs(), u, eta))
+        within(f"out gather {dt}", out, r, b(r, la.bound_out(mags)), M=mags["M"])
+        within(f"probs gather {dt}", probs, la.probs(), b(la.probs(), la.bound_probs()))
         m = torch.rand(B, 1, H, W, device=DEV).to(TDT[dt])
         prev = torch.randn(B, C, H, W, device=DEV).to(TDT[dt])
-        rb, Mb = ref64.blend_ref(r, M, host(prev), host(m))
+        rb, Mb = ref64.blend_ref(r, mags["M"], host(prev), host(m))
         within(f"out gather blend {dt}", F_.local_attn_blend_fwd(s, f, lg, prev, m, k, algo="gather"), rb,
-               ref64.bound_out_gather(rb, Mb, u, eta), M=Mb)
+               b(rb, la.bound_blend(rb, mags, host(prev), host(m))), M=Mb)
         rr = la.bwd(host(s), host(g))
         gs, gf, gl = F_.local_attn_bwd(s, f, lg, g, k, algo="gather")
         assert gs.dtype == s.dtype and gf.dtype == f.dtype and gl.dtype == lg.dtype
-        within(f"grad_source gather {dt}", gs, rr["gs"], ref64.bound_gs_gather(rr["gs"], rr["Mgs"], u, eta), Mgs=rr["Mgs"])
-        within(f"grad_logits gather {dt}", gl, rr["gl"], ref64.bound_gl(rr["gl"], la.probs(), rr["D"], rr["PD"], C, u, eta),
-               D=rr["D"], PD=rr["PD"])
+        within(f"grad_source gather {dt}", gs, rr["gs"], b(rr["gs"], la.bound_gs(rr)), Mgs=rr["Mgs"])
+        within(f"grad_logits gather {dt}", gl, rr["gl"], b(rr["gl"], la.bound_gl(rr, C)), D=rr["D"], PD=rr["PD"])
         fu, feta = (0.0, 0.0) if flow_dt == "fp32" else (u, eta)
-        within(f"grad_flow gather {dt} flow {flow_dt}", gf, rr["gf"], ref64.bound_gf(rr["gf"], rr["Mgf"], C, fu, feta),
+        within(f"grad_flow gather {dt} flow {flow_dt}", gf, rr["gf"], ref64.bound_gather16(rr["gf"], la.bound_gf(rr, C), fu, feta),
                Mgf=rr["Mgf"])
 
 
@@ -177,12 +179,14 @@ def test_block_extract_16bit(F_, dt, flow_dt):
     for kind in ("smooth", "border"):
         s, f, _, _ = make(B, C, Hs, Ws, H, W, k, kind, seed=len(kind) + len(dt), dt=dt, flow_dt=fdt)
         g = torch.randn(B, C, k * H, k * W, device=DEV).to(TDT[dt])
-        r = ref64.block_extract(host(s), host(f), k, host(g))
+        be = ref64_gather.BlockExtract(host(s), host(f), k, host(g), np.float32)
+        r = be.r
         out = F_.block_extract_fwd(s, f, k)
-        within(f"block_extract fwd {dt}", out, r["out"], ref64.bound_be(r["out"], r["M"], u, eta), M=r["M"])
+        within(f"block_extract fwd {dt}", out, r["out"], ref64.bound_gather16(r["out"], be.bound_out(), u, eta), M=r["M"])
         gs, gf = F_.block_extract_bwd(s, f, g, k)
         assert gs.dtype == s.dtype and gf.dtype == f.dtype
-        within(f"block_extract grad_source {dt}", gs, r["gs"], ref64.bound_be(r["gs"], r["Mgs"], u, eta), Mgs=r["Mgs"])
+        within(f"block_extract grad_source {dt}", gs, r["gs"], ref64.bound_gather16(r["gs"], be.bound_gs(), u, eta),
+               Mgs=r["Mgs"])
         fu, feta = (0.0, 0.0) if flow_dt == "fp32" else (u, eta)
         within(f"block_extract grad_flow {dt} flow {flow_dt}", gf, r["gf"],
-               ref64.bound_be_gf(r["gf"], r["Mgf"], k * k * C, fu, feta), Mgf=r["Mgf"])
+               ref64.bound_gather16(r["gf"], be.bound_gf(), fu, feta), Mgf=r["Mgf"])

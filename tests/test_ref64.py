@@ -152,15 +152,20 @@ def test_bounds_accept_emulated_tile_backward_grad_source(case5):
 
 @pytest.mark.parametrize("dt", ["bf16", "fp16"])
 def test_bounds_accept_single_rounding_gather(case5, dt):
+    import ref64_gather
     c = case5
     u, eta = ref64.storage(dt)
     rnd = ref64.round_bf16 if dt == "bf16" else ref64.round_fp16
-    r, la = c["r"], c["la"]
-    worst = [ref64.assert_within("out", rnd(c["out"]), c["out"], ref64.bound_out_gather(c["out"], c["M"], u, eta)),
-             ref64.assert_within("probs", rnd(la.probs()), la.probs(), ref64.bound_probs(la.probs(), u, eta)),
-             ref64.assert_within("gs", rnd(r["gs"]), r["gs"], ref64.bound_gs_gather(r["gs"], r["Mgs"], u, eta)),
-             ref64.assert_within("gl", rnd(r["gl"]), r["gl"], ref64.bound_gl(r["gl"], la.probs(), r["D"], r["PD"], 64, u, eta)),
-             ref64.assert_within("gf", rnd(r["gf"]), r["gf"], ref64.bound_gf(r["gf"], r["Mgf"], 64, u, eta))]
+    g32 = ref64_gather.LocalAttn(c["f"], c["lg"], 5, SHAPE[2], SHAPE[3], np.float32)
+    out, mags = g32.fwd(c["s"])
+    r = g32.bwd(c["s"], c["g"])
+    p = g32.probs()
+    b = lambda y, e32: ref64.bound_gather16(y, e32, u, eta)
+    worst = [ref64.assert_within("out", rnd(out), out, b(out, g32.bound_out(mags))),
+             ref64.assert_within("probs", rnd(p), p, b(p, g32.bound_probs())),
+             ref64.assert_within("gs", rnd(r["gs"]), r["gs"], b(r["gs"], g32.bound_gs(r))),
+             ref64.assert_within("gl", rnd(r["gl"]), r["gl"], b(r["gl"], g32.bound_gl(r, 64))),
+             ref64.assert_within("gf", rnd(r["gf"]), r["gf"], b(r["gf"], g32.bound_gf(r, 64)))]
     assert min(worst) > 0.3
 
 
