@@ -55,6 +55,18 @@ __device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], 
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
+// ------------------------------------------------------------------ named barriers and register reallocation
+// bar.arrive signals without waiting; bar.sync waits until n threads (a multiple of 32) have arrived or synced on the
+// barrier id.  Both order this thread's earlier shared-memory accesses before the accesses of the threads that sync.
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// per-thread register budget of the executing warp (sm_90a, warp-uniform; the kernel's launch bounds fix the starting
+// budget).  A warp that raises its budget waits until other warps of the CTA have released enough.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 __device__ __forceinline__ uint32_t bf16_bits(float v) {
     const __nv_bfloat16 h = __float2bfloat16_rn(v);
     return static_cast<uint32_t>(*reinterpret_cast<const unsigned short*>(&h));
