@@ -187,6 +187,54 @@ int gfla_resample2d_cosine_bwd(const void* in1, const void* in2, const void* tar
                               eps, dtype, accumulate, (cudaStream_t)stream);
 }
 
+// 16-bit storage: the feature maps in dtype (BF16 / F16 only), the flow, stats, grad_in2, grad_in1 and grad_val in fp32
+static inline bool dtype16(int d) { return d == GFLA_BF16 || d == GFLA_F16; }
+
+int gfla_resample2d16_fwd(const void* in1, const void* in2_f32, void* out, int B, int C, int Hi, int Wi, int H, int W, int ks,
+                          int dilation, int dtype, gfla_stream_t stream) {
+    REQ_PTR(in1); REQ_PTR(in2_f32); REQ_PTR(out);
+    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1) return GFLA_E_SHAPE;
+    if (!dtype16(dtype)) return GFLA_E_DTYPE;
+    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2_f32, GFLA_F32); REQ_ALIGN(out, dtype);
+    return resample2d_fwd(in1, in2_f32, out, B, C, Hi, Wi, H, W, ks, dilation, dtype, (cudaStream_t)stream);
+}
+
+int gfla_resample2d16_bwd(const void* in1, const void* in2_f32, const void* grad_out, void* grad_in1_f32, void* grad_in2_f32, int B,
+                          int C, int Hi, int Wi, int H, int W, int ks, int dilation, int dtype, int accumulate, gfla_stream_t stream) {
+    REQ_PTR(in1); REQ_PTR(in2_f32); REQ_PTR(grad_out); REQ_PTR(grad_in1_f32); REQ_PTR(grad_in2_f32);
+    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1) return GFLA_E_SHAPE;
+    if (!dtype16(dtype)) return GFLA_E_DTYPE;
+    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2_f32, GFLA_F32); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_in1_f32, GFLA_F32);
+    REQ_ALIGN(grad_in2_f32, GFLA_F32);
+    return resample2d_bwd(in1, in2_f32, grad_out, grad_in1_f32, grad_in2_f32, B, C, Hi, Wi, H, W, ks, dilation, dtype, accumulate,
+                          (cudaStream_t)stream);
+}
+
+int gfla_resample2d16_cosine_fwd(const void* in1, const void* in2_f32, const void* target, void* cos_out, void* stats_f32, int B, int C,
+                                 int Hi, int Wi, int H, int W, int ks, int dilation, double eps, int dtype, gfla_stream_t stream) {
+    REQ_PTR(in1); REQ_PTR(in2_f32); REQ_PTR(target); REQ_PTR(cos_out); REQ_PTR(stats_f32);
+    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1 || !(eps >= 0)) return GFLA_E_SHAPE;
+    if (!dtype16(dtype)) return GFLA_E_DTYPE;
+    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2_f32, GFLA_F32); REQ_ALIGN(target, dtype); REQ_ALIGN(cos_out, dtype); REQ_ALIGN(stats_f32, GFLA_F32);
+    return resample2d_cos_fwd(in1, in2_f32, target, cos_out, stats_f32, B, C, Hi, Wi, H, W, ks, dilation, eps, dtype, (cudaStream_t)stream);
+}
+
+int gfla_resample2d16_cosine_bwd(const void* in1, const void* in2_f32, const void* target, const void* stats_f32, const void* grad_cos,
+                                 void* grad_in1_f32, void* grad_in2_f32, void* grad_val_f32, void* grad_target, int B, int C, int Hi, int Wi,
+                                 int H, int W, int ks, int dilation, double eps, int dtype, int accumulate, gfla_stream_t stream) {
+    REQ_PTR(in1); REQ_PTR(in2_f32); REQ_PTR(target); REQ_PTR(stats_f32); REQ_PTR(grad_cos); REQ_PTR(grad_in2_f32);
+    if (grad_in1_f32 != nullptr && grad_val_f32 == nullptr) return GFLA_E_NULL;
+    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1 || !(eps >= 0)) return GFLA_E_SHAPE;
+    if (!dtype16(dtype)) return GFLA_E_DTYPE;
+    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2_f32, GFLA_F32); REQ_ALIGN(target, dtype); REQ_ALIGN(stats_f32, GFLA_F32); REQ_ALIGN(grad_cos, dtype);
+    REQ_ALIGN(grad_in2_f32, GFLA_F32);
+    if (grad_in1_f32 != nullptr) { REQ_ALIGN(grad_in1_f32, GFLA_F32); }
+    if (grad_val_f32 != nullptr) { REQ_ALIGN(grad_val_f32, GFLA_F32); }
+    if (grad_target != nullptr) { REQ_ALIGN(grad_target, dtype); }
+    return resample2d_cos_bwd(in1, in2_f32, target, stats_f32, grad_cos, grad_in1_f32, grad_in2_f32, grad_val_f32, grad_target, B, C, Hi, Wi,
+                              H, W, ks, dilation, eps, dtype, accumulate, (cudaStream_t)stream);
+}
+
 static int local_attn_fwd_any(const void* source, const void* flow, const void* logits, void* out, void* probs,
                               const void* prev, const void* mask, int B, int C, int Hs, int Ws, int H, int W, int k, int dtype,
                               int flow_dtype, int layout, int algo, gfla_stream_t stream) {

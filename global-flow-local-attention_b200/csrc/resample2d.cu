@@ -24,6 +24,8 @@
 //     derives the three gradients from them.
 // Compiled with -fmad=false: the fp32/fp64 forward is bit-identical to the
 // (uncontracted) CPU oracle up to the last-ulp behaviour of exp().
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace gfla {
@@ -111,10 +113,14 @@ __device__ __forceinline__ A rs_weight_sum(const RsTaps<A, NT>& t) {
     return sum;
 }
 
-template <typename A, int NT>
-__global__ void __launch_bounds__(128)
-k_resample2d_fwd(const A* __restrict__ in1, const A* __restrict__ in2, A* __restrict__ out, int B, int C, int Hi, int Wi,
-                 int H, int W, int dil, int c_per_slice) {
+// The per-pixel bodies below are templates over the storage type T of the feature maps (in1, out, grad_out, target, cos,
+// grad_cos, grad_target) and the arithmetic type A.  The fp32 / fp64 kernels run them with T = A.  The 16-bit kernels
+// (k_resample2d16_*) run them with T = bf16 / fp16 and A = float: every 16-bit value is widened on load, the arithmetic
+// and the taps are exactly the fp32 kernel's on the widened values (in2, stats, grad_in2 and the grad_in1 / grad_val
+// buffers stay fp32), and each 16-bit output is rounded once, at its store.
+template <typename T, typename A, int NT>
+__device__ __forceinline__ void rs_fwd(const T* __restrict__ in1, const A* __restrict__ in2, T* __restrict__ out, int B, int C,
+                                       int Hi, int Wi, int H, int W, int dil, int c_per_slice) {
     const RsPixel px = rs_pixel<4>(H, W);
     if (!px.active) return;
     const int x = px.x, y = px.y, b = px.b;
@@ -132,15 +138,29 @@ k_resample2d_fwd(const A* __restrict__ in1, const A* __restrict__ in2, A* __rest
     const A sum = rs_weight_sum<A, NT>(t);
     const long long ipl = (long long)Hi * Wi, opl = (long long)H * W;
     const int c0 = blockIdx.y * c_per_slice, c1 = min(C, c0 + c_per_slice);
-    const A* s = in1 + ((long long)b * C + c0) * ipl;
-    A* o = out + ((long long)b * C + c0) * opl + (long long)y * W + x;
+    const T* s = in1 + ((long long)b * C + c0) * ipl;
+    T* o = out + ((long long)b * C + c0) * opl + (long long)y * W + x;
 #pragma unroll 4
     for (int c = c0; c < c1; ++c, s += ipl, o += opl) {   // unrolled: 4 channels x taps of independent loads in flight
         A val = static_cast<A>(0);
 #pragma unroll
-        for (int q = 0; q < NT * NT * 4; ++q) val += w[q] * s[t.off[q]];
-        *o = static_cast<A>(safe_div<A>(val, sum));
+        for (int q = 0; q < NT * NT * 4; ++q) val += w[q] * static_cast<A>(s[t.off[q]]);
+        *o = static_cast<T>(static_cast<A>(safe_div<A>(val, sum)));
     }
+}
+
+template <typename A, int NT>
+__global__ void __launch_bounds__(128)
+k_resample2d_fwd(const A* __restrict__ in1, const A* __restrict__ in2, A* __restrict__ out, int B, int C, int Hi, int Wi,
+                 int H, int W, int dil, int c_per_slice) {
+    rs_fwd<A, A, NT>(in1, in2, out, B, C, Hi, Wi, H, W, dil, c_per_slice);
+}
+
+template <typename T, int NT>
+__global__ void __launch_bounds__(128)
+k_resample2d16_fwd(const T* __restrict__ in1, const float* __restrict__ in2, T* __restrict__ out, int B, int C, int Hi, int Wi,
+                   int H, int W, int dil, int c_per_slice) {
+    rs_fwd<T, float, NT>(in1, in2, out, B, C, Hi, Wi, H, W, dil, c_per_slice);
 }
 
 // grad_input1: a scatter of 4*(ks/2)^2 weighted copies of grad_out per (pixel, channel).  A warp is a 32-pixel run of one
@@ -148,10 +168,10 @@ k_resample2d_fwd(const A* __restrict__ in1, const A* __restrict__ in2, A* __rest
 // tap is clamped, lane L's contribution to column (x_L + shift + co) is exactly what lane L+co accumulates for its
 // own centre column: the (2*ks/2)^2 scalar atomics per element collapse to one red.global per tap ROW per lane
 // (plus the few taps that leave the warp's 32 columns) after a register-level exchange with __shfl_sync.
-template <typename A, int NT>
-__global__ void __launch_bounds__(128)
-k_resample2d_bwd_in1(const A* __restrict__ in2, const A* __restrict__ gout, A* __restrict__ gin1, int B, int C, int Hi,
-                     int Wi, int H, int W, int dil, int c_per_slice) {
+// grad_in1 is summed in A: a 16-bit call scatters into an fp32 buffer that the caller narrows once (gfla_convert).
+template <typename T, typename A, int NT>
+__device__ __forceinline__ void rs_bwd_in1(const A* __restrict__ in2, const T* __restrict__ gout, A* __restrict__ gin1, int B, int C,
+                                           int Hi, int Wi, int H, int W, int dil, int c_per_slice) {
     const RsPixel px = rs_pixel<4>(H, W);
     const bool active = px.active;
     const int x = min(px.x, W - 1), y = min(px.y, H - 1), b = px.b;   // inactive lanes stay alive for the warp shuffles
@@ -170,7 +190,7 @@ k_resample2d_bwd_in1(const A* __restrict__ in2, const A* __restrict__ gout, A* _
     const long long ipl = (long long)Hi * Wi, opl = (long long)H * W;
     const int c0 = blockIdx.y * c_per_slice, c1 = min(C, c0 + c_per_slice);
     A* gi = gin1 + ((long long)b * C + c0) * ipl;
-    const A* go = gout + ((long long)b * C + c0) * opl + (long long)y * W + x;
+    const T* go = gout + ((long long)b * C + c0) * opl + (long long)y * W + x;
 
     bool fast = false;
     if (NT <= 2) {
@@ -201,7 +221,7 @@ k_resample2d_bwd_in1(const A* __restrict__ in2, const A* __restrict__ gout, A* _
             }
         const int centre = (t.fly - (NT - 1)) * Wi + t.flx;      // first tap row, this lane's centre column
         for (int c = c0; c < c1; ++c, gi += ipl, go += opl) {
-            const double g = static_cast<double>(*go);
+            const double g = static_cast<double>(static_cast<A>(*go));
 #pragma unroll
             for (int ri = 0; ri < N2; ++ri) {
                 A acc = static_cast<A>(0);
@@ -221,10 +241,24 @@ k_resample2d_bwd_in1(const A* __restrict__ in2, const A* __restrict__ gout, A* _
     if (!active) return;
 #pragma unroll 4
     for (int c = c0; c < c1; ++c, gi += ipl, go += opl) {
-        const double g = static_cast<double>(*go);
+        const double g = static_cast<double>(static_cast<A>(*go));
 #pragma unroll
         for (int q = 0; q < NT * NT * 4; ++q) atomicAdd(gi + t.off[q], static_cast<A>(wn[q] * g));
     }
+}
+
+template <typename A, int NT>
+__global__ void __launch_bounds__(128)
+k_resample2d_bwd_in1(const A* __restrict__ in2, const A* __restrict__ gout, A* __restrict__ gin1, int B, int C, int Hi,
+                     int Wi, int H, int W, int dil, int c_per_slice) {
+    rs_bwd_in1<A, A, NT>(in2, gout, gin1, B, C, Hi, Wi, H, W, dil, c_per_slice);
+}
+
+template <typename T, int NT>
+__global__ void __launch_bounds__(128)
+k_resample2d16_bwd_in1(const float* __restrict__ in2, const T* __restrict__ gout, float* __restrict__ gin1, int B, int C, int Hi,
+                       int Wi, int H, int W, int dil, int c_per_slice) {
+    rs_bwd_in1<T, float, NT>(in2, gout, gin1, B, C, Hi, Wi, H, W, dil, c_per_slice);
 }
 
 // d/d(dx, dy, sigma) of one pixel from its corner dot products D[q] = sum_c g[c] * in1[c, tap q]
@@ -263,10 +297,9 @@ __device__ __forceinline__ void rs_in2_store(const RsTaps<A, NT>& t, A sum, cons
     }
 }
 
-template <typename A, int NT>
-__global__ void __launch_bounds__(128)
-k_resample2d_bwd_in2(const A* __restrict__ in1, const A* __restrict__ in2, const A* __restrict__ gout,
-                     A* __restrict__ gin2, int B, int C, int Hi, int Wi, int H, int W, int dil, int accumulate) {
+template <typename T, typename A, int NT>
+__device__ __forceinline__ void rs_bwd_in2(const T* __restrict__ in1, const A* __restrict__ in2, const T* __restrict__ gout,
+                                           A* __restrict__ gin2, int B, int C, int Hi, int Wi, int H, int W, int dil, int accumulate) {
     const RsPixel px = rs_pixel<4>(H, W);
     if (!px.active) return;
     const int x = px.x, y = px.y, b = px.b;
@@ -278,15 +311,29 @@ k_resample2d_bwd_in2(const A* __restrict__ in1, const A* __restrict__ in2, const
 #pragma unroll
     for (int q = 0; q < NT * NT * 4; ++q) D[q] = static_cast<A>(0);
     const long long ipl = (long long)Hi * Wi, opl = (long long)H * W;
-    const A* s = in1 + (long long)b * C * ipl;
-    const A* go = gout + (long long)b * C * opl + (long long)y * W + x;
+    const T* s = in1 + (long long)b * C * ipl;
+    const T* go = gout + (long long)b * C * opl + (long long)y * W + x;
 #pragma unroll 4
     for (int c = 0; c < C; ++c, s += ipl, go += opl) {
-        const A g = *go;
+        const A g = static_cast<A>(*go);
 #pragma unroll
-        for (int q = 0; q < NT * NT * 4; ++q) D[q] += g * s[t.off[q]];
+        for (int q = 0; q < NT * NT * 4; ++q) D[q] += g * static_cast<A>(s[t.off[q]]);
     }
     rs_in2_store<A, NT>(t, sum, D, gin2 + (long long)b * 3 * opl + (long long)y * W + x, opl, accumulate);
+}
+
+template <typename A, int NT>
+__global__ void __launch_bounds__(128)
+k_resample2d_bwd_in2(const A* __restrict__ in1, const A* __restrict__ in2, const A* __restrict__ gout,
+                     A* __restrict__ gin2, int B, int C, int Hi, int Wi, int H, int W, int dil, int accumulate) {
+    rs_bwd_in2<A, A, NT>(in1, in2, gout, gin2, B, C, Hi, Wi, H, W, dil, accumulate);
+}
+
+template <typename T, int NT>
+__global__ void __launch_bounds__(128)
+k_resample2d16_bwd_in2(const T* __restrict__ in1, const float* __restrict__ in2, const T* __restrict__ gout,
+                       float* __restrict__ gin2, int B, int C, int Hi, int Wi, int H, int W, int dil, int accumulate) {
+    rs_bwd_in2<T, float, NT>(in1, in2, gout, gin2, B, C, Hi, Wi, H, W, dil, accumulate);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -298,10 +345,10 @@ k_resample2d_bwd_in2(const A* __restrict__ in1, const A* __restrict__ in2, const
 // stats[b, 0..2, y, x] = (v.t, |v|, |t|) are kept for the backward.
 // TS > 1: the 4 warps of a CTA are TS channel slices of ONE 32-pixel row segment (feature maps of a loss are small: a thread per
 // pixel alone leaves the SMs with a handful of warps each, walking C channels one after the other); the partial sums meet in shared memory.
-template <typename A, int NT, int TS>
-__global__ void __launch_bounds__(128)
-k_resample2d_cos_fwd(const A* __restrict__ in1, const A* __restrict__ in2, const A* __restrict__ target, A* __restrict__ cos_out,
-                     A* __restrict__ stats, int B, int C, int Hi, int Wi, int H, int W, int dil, A eps) {
+template <typename T, typename A, int NT, int TS>
+__device__ __forceinline__ void rs_cos_fwd(const T* __restrict__ in1, const A* __restrict__ in2, const T* __restrict__ target,
+                                           T* __restrict__ cos_out, A* __restrict__ stats, int B, int C, int Hi, int Wi, int H, int W,
+                                           int dil, A eps) {
     constexpr int TH = 4 / TS;                                   // pixel rows per CTA
     __shared__ A part[TS > 1 ? 3 * TS * 32 * TH : 1];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -323,16 +370,16 @@ k_resample2d_cos_fwd(const A* __restrict__ in1, const A* __restrict__ in2, const
     const A sum = rs_weight_sum<A, NT>(t);
     const long long ipl = (long long)Hi * Wi, opl = (long long)H * W, pix = (long long)y * W + x;
     const int cs = (C + TS - 1) / TS, c0 = slice * cs, c1 = min(C, c0 + cs);
-    const A* s = in1 + ((long long)b * C + c0) * ipl;
-    const A* tg = target + ((long long)b * C + c0) * opl + pix;
+    const T* s = in1 + ((long long)b * C + c0) * ipl;
+    const T* tg = target + ((long long)b * C + c0) * opl + pix;
     A dot = static_cast<A>(0), vv = static_cast<A>(0), tt = static_cast<A>(0);
 #pragma unroll 4
     for (int c = c0; c < c1; ++c, s += ipl, tg += opl) {
         A val = static_cast<A>(0);
 #pragma unroll
-        for (int q = 0; q < NT * NT * 4; ++q) val += w[q] * s[t.off[q]];
-        const A v = static_cast<A>(safe_div<A>(val, sum));        // exactly k_resample2d_fwd's output element
-        const A tc = *tg;
+        for (int q = 0; q < NT * NT * 4; ++q) val += w[q] * static_cast<A>(s[t.off[q]]);
+        const A v = static_cast<A>(safe_div<A>(val, sum));        // exactly k_resample2d_fwd's output element (before its 16-bit store)
+        const A tc = static_cast<A>(*tg);
         dot += v * tc; vv += v * v; tt += tc * tc;
     }
     if (TS > 1) {
@@ -348,9 +395,23 @@ k_resample2d_cos_fwd(const A* __restrict__ in1, const A* __restrict__ in2, const
         }
     }
     const A nv = sqrt(vv), nt = sqrt(tt);
-    cos_out[(long long)b * opl + pix] = dot / (max(nv, eps) * max(nt, eps));
-    A* st = stats + (long long)b * 3 * opl + pix;
-    st[0] = dot; st[opl] = nv; st[2 * opl] = nt;
+    cos_out[(long long)b * opl + pix] = static_cast<T>(dot / (max(nv, eps) * max(nt, eps)));
+    A* sp = stats + (long long)b * 3 * opl + pix;
+    sp[0] = dot; sp[opl] = nv; sp[2 * opl] = nt;
+}
+
+template <typename A, int NT, int TS>
+__global__ void __launch_bounds__(128)
+k_resample2d_cos_fwd(const A* __restrict__ in1, const A* __restrict__ in2, const A* __restrict__ target, A* __restrict__ cos_out,
+                     A* __restrict__ stats, int B, int C, int Hi, int Wi, int H, int W, int dil, A eps) {
+    rs_cos_fwd<A, A, NT, TS>(in1, in2, target, cos_out, stats, B, C, Hi, Wi, H, W, dil, eps);
+}
+
+template <typename T, int NT, int TS>
+__global__ void __launch_bounds__(128)
+k_resample2d16_cos_fwd(const T* __restrict__ in1, const float* __restrict__ in2, const T* __restrict__ target, T* __restrict__ cos_out,
+                       float* __restrict__ stats, int B, int C, int Hi, int Wi, int H, int W, int dil, float eps) {
+    rs_cos_fwd<T, float, NT, TS>(in1, in2, target, cos_out, stats, B, C, Hi, Wi, H, W, dil, eps);
 }
 
 // Backward of the fused op for one pixel, one pass over the channels: the warped value v_c is rebuilt from the taps that are in
@@ -358,11 +419,12 @@ k_resample2d_cos_fwd(const A* __restrict__ in1, const A* __restrict__ in2, const
 // g_c * tap -- so the flow gradient (the one PerceptualCorrectness trains through) costs one read of the source and the
 // target and writes 3 floats per pixel.  grad_val (optional) receives g_c for the grad_input1 scatter (k_resample2d_bwd_in1 runs on
 // it afterwards; VGG features of data carry no gradient in the reference's use), grad_target (optional) dcos/dt_c * grad_cos.
-template <typename A, int NT, int TS>
-__global__ void __launch_bounds__(128)
-k_resample2d_cos_bwd(const A* __restrict__ in1, const A* __restrict__ in2, const A* __restrict__ target, const A* __restrict__ stats,
-                     const A* __restrict__ gcos, A* __restrict__ gin2, A* __restrict__ gval, A* __restrict__ gtarget, int B, int C,
-                     int Hi, int Wi, int H, int W, int dil, A eps, int accumulate) {
+// grad_val is A (the fp32 buffer of a 16-bit call feeds the fp32 k_resample2d_bwd_in1), grad_target T
+template <typename T, typename A, int NT, int TS>
+__device__ __forceinline__ void rs_cos_bwd(const T* __restrict__ in1, const A* __restrict__ in2, const T* __restrict__ target,
+                                           const A* __restrict__ stats, const T* __restrict__ gcos, A* __restrict__ gin2,
+                                           A* __restrict__ gval, T* __restrict__ gtarget, int B, int C, int Hi, int Wi, int H, int W,
+                                           int dil, A eps, int accumulate) {
     constexpr int TH = 4 / TS, NQ = NT * NT * 4;
     __shared__ A part[TS > 1 ? NQ * TS * 32 * TH : 1];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -385,35 +447,35 @@ k_resample2d_cos_bwd(const A* __restrict__ in1, const A* __restrict__ in2, const
     for (int q = 0; q < NQ; ++q) D[q] = static_cast<A>(0);
     const A sum = rs_weight_sum<A, NT>(t);
     const long long ipl = (long long)Hi * Wi, opl = (long long)H * W, pix = (long long)y * W + x;
-    const A* st = stats + (long long)b * 3 * opl + pix;
-    const A dot = st[0], nv = st[opl], nt = st[2 * opl];
-    const A a = max(nv, eps), bb = max(nt, eps), g = gcos[(long long)b * opl + pix];
+    const A* sp = stats + (long long)b * 3 * opl + pix;
+    const A dot = sp[0], nv = sp[opl], nt = sp[2 * opl];
+    const A a = max(nv, eps), bb = max(nt, eps), g = static_cast<A>(gcos[(long long)b * opl + pix]);
     // cos = dot / (a * bb);  da/dv_c = v_c / |v| above the clamp, 0 below it
     const A k1 = g / (a * bb);
     const A k2v = nv > eps ? g * dot / (a * a * bb * nv) : static_cast<A>(0);
     const A k2t = nt > eps ? g * dot / (a * bb * bb * nt) : static_cast<A>(0);
     const int cs = (C + TS - 1) / TS, c0 = slice * cs, c1 = min(C, c0 + cs);
-    const A* s = in1 + ((long long)b * C + c0) * ipl;
+    const T* s = in1 + ((long long)b * C + c0) * ipl;
     const long long o0 = ((long long)b * C + c0) * opl + pix;
-    const A* tg = target + o0;
+    const T* tg = target + o0;
     const bool live = px.active;                                  // inactive lanes only keep the CTA barrier company
     A* gv = gval != nullptr && live ? gval + o0 : nullptr;
-    A* gt = gtarget != nullptr && live ? gtarget + o0 : nullptr;
+    T* gt = gtarget != nullptr && live ? gtarget + o0 : nullptr;
 #pragma unroll 2
     for (int c = c0; c < c1; ++c, s += ipl, tg += opl) {
         A tap[NQ];
         A val = static_cast<A>(0);
 #pragma unroll
-        for (int q = 0; q < NQ; ++q) { tap[q] = s[t.off[q]]; val += w[q] * tap[q]; }
+        for (int q = 0; q < NQ; ++q) { tap[q] = static_cast<A>(s[t.off[q]]); val += w[q] * tap[q]; }
         const A v = static_cast<A>(safe_div<A>(val, sum));
-        const A tc = *tg;
+        const A tc = static_cast<A>(*tg);
         const A gc = k1 * tc - k2v * v;
 #pragma unroll
         for (int q = 0; q < NQ; ++q) D[q] += gc * tap[q];
         if (gv != nullptr) gv[(long long)(c - c0) * opl] = gc;
         if (gt != nullptr) {
             const A d = k1 * v - k2t * tc;
-            gt[(long long)(c - c0) * opl] = accumulate ? gt[(long long)(c - c0) * opl] + d : d;
+            gt[(long long)(c - c0) * opl] = static_cast<T>(accumulate ? static_cast<A>(gt[(long long)(c - c0) * opl]) + d : d);
         }
     }
     if (TS > 1) {
@@ -434,27 +496,60 @@ k_resample2d_cos_bwd(const A* __restrict__ in1, const A* __restrict__ in2, const
     rs_in2_store<A, NT>(t, sum, D, gin2 + (long long)b * 3 * opl + pix, opl, accumulate);
 }
 
-template <typename A, int NT>
+template <typename A, int NT, int TS>
+__global__ void __launch_bounds__(128)
+k_resample2d_cos_bwd(const A* __restrict__ in1, const A* __restrict__ in2, const A* __restrict__ target, const A* __restrict__ stats,
+                     const A* __restrict__ gcos, A* __restrict__ gin2, A* __restrict__ gval, A* __restrict__ gtarget, int B, int C,
+                     int Hi, int Wi, int H, int W, int dil, A eps, int accumulate) {
+    rs_cos_bwd<A, A, NT, TS>(in1, in2, target, stats, gcos, gin2, gval, gtarget, B, C, Hi, Wi, H, W, dil, eps, accumulate);
+}
+
+template <typename T, int NT, int TS>
+__global__ void __launch_bounds__(128)
+k_resample2d16_cos_bwd(const T* __restrict__ in1, const float* __restrict__ in2, const T* __restrict__ target,
+                       const float* __restrict__ stats, const T* __restrict__ gcos, float* __restrict__ gin2, float* __restrict__ gval,
+                       T* __restrict__ gtarget, int B, int C, int Hi, int Wi, int H, int W, int dil, float eps, int accumulate) {
+    rs_cos_bwd<T, float, NT, TS>(in1, in2, target, stats, gcos, gin2, gval, gtarget, B, C, Hi, Wi, H, W, dil, eps, accumulate);
+}
+
+// The kernel a launch of storage type T (arithmetic A) runs: the fp32 / fp64 instance when T == A, the 16-bit one otherwise.
+template <typename T, typename A, int NT> constexpr auto rs_fwd_kernel() {
+    if constexpr (std::is_same_v<T, A>) return k_resample2d_fwd<A, NT>; else return k_resample2d16_fwd<T, NT>;
+}
+template <typename T, typename A, int NT> constexpr auto rs_bwd_in1_kernel() {
+    if constexpr (std::is_same_v<T, A>) return k_resample2d_bwd_in1<A, NT>; else return k_resample2d16_bwd_in1<T, NT>;
+}
+template <typename T, typename A, int NT> constexpr auto rs_bwd_in2_kernel() {
+    if constexpr (std::is_same_v<T, A>) return k_resample2d_bwd_in2<A, NT>; else return k_resample2d16_bwd_in2<T, NT>;
+}
+template <typename T, typename A, int NT, int TS> constexpr auto rs_cos_fwd_kernel() {
+    if constexpr (std::is_same_v<T, A>) return k_resample2d_cos_fwd<A, NT, TS>; else return k_resample2d16_cos_fwd<T, NT, TS>;
+}
+template <typename T, typename A, int NT, int TS> constexpr auto rs_cos_bwd_kernel() {
+    if constexpr (std::is_same_v<T, A>) return k_resample2d_cos_bwd<A, NT, TS>; else return k_resample2d16_cos_bwd<T, NT, TS>;
+}
+
+template <typename T, typename A, int NT>
 static int rs_launch_fwd(const void* in1, const void* in2, void* out, int B, int C, int Hi, int Wi, int H, int W, int dil,
                          cudaStream_t st_) {
     const long long total = (long long)B * H * W;
     const int threads = 128, slices0 = channel_splits(total, C, threads), cps = (C + slices0 - 1) / slices0;
     dim3 grid((unsigned)rs_tiles<4>(B, H, W), (unsigned)((C + cps - 1) / cps));
-    k_resample2d_fwd<A, NT><<<grid, threads, 0, st_>>>((const A*)in1, (const A*)in2, (A*)out, B, C, Hi, Wi, H, W, dil, cps);
+    rs_fwd_kernel<T, A, NT>()<<<grid, threads, 0, st_>>>((const T*)in1, (const A*)in2, (T*)out, B, C, Hi, Wi, H, W, dil, cps);
     return launch_status();
 }
 
-template <typename A, int NT>
+template <typename T, typename A, int NT>
 static int rs_launch_bwd(const void* in1, const void* in2, const void* gout, void* gin1, void* gin2, int B, int C, int Hi,
                          int Wi, int H, int W, int dil, int accumulate, cudaStream_t st_) {
     const long long total = (long long)B * H * W;
     const int threads = 128, slices0 = channel_splits(total, C, threads), cps = (C + slices0 - 1) / slices0;
     dim3 grid((unsigned)rs_tiles<4>(B, H, W), (unsigned)((C + cps - 1) / cps));
-    k_resample2d_bwd_in1<A, NT><<<grid, threads, 0, st_>>>((const A*)in2, (const A*)gout, (A*)gin1, B, C, Hi, Wi, H, W, dil, cps);
+    rs_bwd_in1_kernel<T, A, NT>()<<<grid, threads, 0, st_>>>((const A*)in2, (const T*)gout, (A*)gin1, B, C, Hi, Wi, H, W, dil, cps);
     int e = launch_status();
     if (e) return e;
-    k_resample2d_bwd_in2<A, NT><<<(unsigned)rs_tiles<4>(B, H, W), 128, 0, st_>>>(
-        (const A*)in1, (const A*)in2, (const A*)gout, (A*)gin2, B, C, Hi, Wi, H, W, dil, accumulate);
+    rs_bwd_in2_kernel<T, A, NT>()<<<(unsigned)rs_tiles<4>(B, H, W), 128, 0, st_>>>(
+        (const T*)in1, (const A*)in2, (const T*)gout, (A*)gin2, B, C, Hi, Wi, H, W, dil, accumulate);
     return launch_status();
 }
 
@@ -464,75 +559,83 @@ static inline int rs_cos_slices(int B, int C, int H, int W) {
     return (C >= 64 && (long long)B * H * W < (long long)sm_count() * 1024) ? 4 : 1;
 }
 
-template <typename A, int NT>
+template <typename T, typename A, int NT>
 static int rs_launch_cos_fwd(const void* in1, const void* in2, const void* target, void* cos_out, void* stats, int B, int C, int Hi,
                              int Wi, int H, int W, int dil, double eps, cudaStream_t st_) {
     bool sliced = false;
     if constexpr (NT <= 2) sliced = rs_cos_slices(B, C, H, W) == 4;      // (larger windows: the partial sums would not fit static shared memory)
     if constexpr (NT <= 2) if (sliced)
-        k_resample2d_cos_fwd<A, NT, 4><<<(unsigned)rs_tiles<1>(B, H, W), 128, 0, st_>>>((const A*)in1, (const A*)in2, (const A*)target, (A*)cos_out,
-                                                                                        (A*)stats, B, C, Hi, Wi, H, W, dil, static_cast<A>(eps));
+        rs_cos_fwd_kernel<T, A, NT, 4>()<<<(unsigned)rs_tiles<1>(B, H, W), 128, 0, st_>>>((const T*)in1, (const A*)in2, (const T*)target, (T*)cos_out,
+                                                                                          (A*)stats, B, C, Hi, Wi, H, W, dil, static_cast<A>(eps));
     if (!sliced)
-        k_resample2d_cos_fwd<A, NT, 1><<<(unsigned)rs_tiles<4>(B, H, W), 128, 0, st_>>>((const A*)in1, (const A*)in2, (const A*)target, (A*)cos_out,
-                                                                                        (A*)stats, B, C, Hi, Wi, H, W, dil, static_cast<A>(eps));
+        rs_cos_fwd_kernel<T, A, NT, 1>()<<<(unsigned)rs_tiles<4>(B, H, W), 128, 0, st_>>>((const T*)in1, (const A*)in2, (const T*)target, (T*)cos_out,
+                                                                                          (A*)stats, B, C, Hi, Wi, H, W, dil, static_cast<A>(eps));
     return launch_status();
 }
 
-template <typename A, int NT>
+template <typename T, typename A, int NT>
 static int rs_launch_cos_bwd(const void* in1, const void* in2, const void* target, const void* stats, const void* gcos, void* gin1,
                              void* gin2, void* gval, void* gtarget, int B, int C, int Hi, int Wi, int H, int W, int dil, double eps,
                              int accumulate, cudaStream_t st_) {
     bool sliced = false;
     if constexpr (NT <= 2) sliced = rs_cos_slices(B, C, H, W) == 4;
     if constexpr (NT <= 2) if (sliced)
-        k_resample2d_cos_bwd<A, NT, 4><<<(unsigned)rs_tiles<1>(B, H, W), 128, 0, st_>>>(
-            (const A*)in1, (const A*)in2, (const A*)target, (const A*)stats, (const A*)gcos, (A*)gin2, (A*)gval, (A*)gtarget, B, C, Hi, Wi,
+        rs_cos_bwd_kernel<T, A, NT, 4>()<<<(unsigned)rs_tiles<1>(B, H, W), 128, 0, st_>>>(
+            (const T*)in1, (const A*)in2, (const T*)target, (const A*)stats, (const T*)gcos, (A*)gin2, (A*)gval, (T*)gtarget, B, C, Hi, Wi,
             H, W, dil, static_cast<A>(eps), accumulate);
     if (!sliced)
-        k_resample2d_cos_bwd<A, NT, 1><<<(unsigned)rs_tiles<4>(B, H, W), 128, 0, st_>>>(
-            (const A*)in1, (const A*)in2, (const A*)target, (const A*)stats, (const A*)gcos, (A*)gin2, (A*)gval, (A*)gtarget, B, C, Hi, Wi,
+        rs_cos_bwd_kernel<T, A, NT, 1>()<<<(unsigned)rs_tiles<4>(B, H, W), 128, 0, st_>>>(
+            (const T*)in1, (const A*)in2, (const T*)target, (const A*)stats, (const T*)gcos, (A*)gin2, (A*)gval, (T*)gtarget, B, C, Hi, Wi,
             H, W, dil, static_cast<A>(eps), accumulate);
     int e = launch_status();
     if (e || gin1 == nullptr) return e;
     const long long total = (long long)B * H * W;
     const int threads = 128, slices0 = channel_splits(total, C, threads), cps = (C + slices0 - 1) / slices0;
     dim3 grid((unsigned)rs_tiles<4>(B, H, W), (unsigned)((C + cps - 1) / cps));
+    // grad_val is A-typed whatever T is: the scatter is the fp32 / fp64 instance
     k_resample2d_bwd_in1<A, NT><<<grid, threads, 0, st_>>>((const A*)in2, (const A*)gval, (A*)gin1, B, C, Hi, Wi, H, W, dil, cps);
     return launch_status();
 }
 
-#define GFLA_RS_DISPATCH(A_, fn, ...)                          \
+#define GFLA_RS_DISPATCH(T_, A_, fn, ...)                      \
     switch (ks / 2) {                                          \
-        case 1: return fn<A_, 1>(__VA_ARGS__);                 \
-        case 2: return fn<A_, 2>(__VA_ARGS__);                 \
-        case 3: return fn<A_, 3>(__VA_ARGS__);                 \
-        case 4: return fn<A_, 4>(__VA_ARGS__);                 \
+        case 1: return fn<T_, A_, 1>(__VA_ARGS__);             \
+        case 2: return fn<T_, A_, 2>(__VA_ARGS__);             \
+        case 3: return fn<T_, A_, 3>(__VA_ARGS__);             \
+        case 4: return fn<T_, A_, 4>(__VA_ARGS__);             \
         default: return GFLA_E_SHAPE;                          \
     }
 
+// F32 / F64 run the T = A kernels, BF16 / F16 (the gfla_resample2d16_* entry points) the 16-bit ones with A = float
+#define GFLA_RS_DTYPES(dtype, fn, ...)                                                                           \
+    switch (dtype) {                                                                                             \
+        case GFLA_F32: { GFLA_RS_DISPATCH(float, float, fn, __VA_ARGS__) }                                       \
+        case GFLA_F64: { GFLA_RS_DISPATCH(double, double, fn, __VA_ARGS__) }                                     \
+        case GFLA_BF16: { GFLA_RS_DISPATCH(__nv_bfloat16, float, fn, __VA_ARGS__) }                              \
+        case GFLA_F16: { GFLA_RS_DISPATCH(__half, float, fn, __VA_ARGS__) }                                      \
+        default: return GFLA_E_DTYPE;                                                                            \
+    }
+
+// element size of grad_in1: a 16-bit call sums it in fp32
+static inline size_t rs_gin1_bytes(int dtype) { return dtype == GFLA_BF16 || dtype == GFLA_F16 ? 4 : elem_size(dtype); }
+
 int resample2d_fwd(const void* in1, const void* in2, void* out, int B, int C, int Hi, int Wi, int H, int W, int ks,
                    int dil, int dtype, cudaStream_t st_) {
-    if (dtype == GFLA_F32) { GFLA_RS_DISPATCH(float, rs_launch_fwd, in1, in2, out, B, C, Hi, Wi, H, W, dil, st_) }
-    if (dtype == GFLA_F64) { GFLA_RS_DISPATCH(double, rs_launch_fwd, in1, in2, out, B, C, Hi, Wi, H, W, dil, st_) }
-    return GFLA_E_DTYPE;
+    GFLA_RS_DTYPES(dtype, rs_launch_fwd, in1, in2, out, B, C, Hi, Wi, H, W, dil, st_)
 }
 
 int resample2d_bwd(const void* in1, const void* in2, const void* gout, void* gin1, void* gin2, int B, int C, int Hi,
                    int Wi, int H, int W, int ks, int dil, int dtype, int accumulate, cudaStream_t st_) {
     if (!accumulate) {
-        const int e = zero_async(gin1, (size_t)B * C * Hi * Wi * elem_size(dtype), st_);
+        const int e = zero_async(gin1, (size_t)B * C * Hi * Wi * rs_gin1_bytes(dtype), st_);
         if (e != GFLA_OK) return e;
     }
-    if (dtype == GFLA_F32) { GFLA_RS_DISPATCH(float, rs_launch_bwd, in1, in2, gout, gin1, gin2, B, C, Hi, Wi, H, W, dil, accumulate, st_) }
-    if (dtype == GFLA_F64) { GFLA_RS_DISPATCH(double, rs_launch_bwd, in1, in2, gout, gin1, gin2, B, C, Hi, Wi, H, W, dil, accumulate, st_) }
-    return GFLA_E_DTYPE;
+    GFLA_RS_DTYPES(dtype, rs_launch_bwd, in1, in2, gout, gin1, gin2, B, C, Hi, Wi, H, W, dil, accumulate, st_)
 }
 
 int resample2d_cos_fwd(const void* in1, const void* in2, const void* target, void* cos_out, void* stats, int B, int C, int Hi, int Wi,
                        int H, int W, int ks, int dil, double eps, int dtype, cudaStream_t st_) {
-    if (dtype == GFLA_F32) { GFLA_RS_DISPATCH(float, rs_launch_cos_fwd, in1, in2, target, cos_out, stats, B, C, Hi, Wi, H, W, dil, eps, st_) }
-    if (dtype == GFLA_F64) { GFLA_RS_DISPATCH(double, rs_launch_cos_fwd, in1, in2, target, cos_out, stats, B, C, Hi, Wi, H, W, dil, eps, st_) }
-    return GFLA_E_DTYPE;
+    GFLA_RS_DTYPES(dtype, rs_launch_cos_fwd, in1, in2, target, cos_out, stats, B, C, Hi, Wi, H, W, dil, eps, st_)
 }
 
 // grad_in1 != nullptr needs grad_val (a [B,C,H,W] scratch tensor of the caller); accumulate = 0 zero-fills grad_in1 first
@@ -540,12 +643,10 @@ int resample2d_cos_bwd(const void* in1, const void* in2, const void* target, con
                        void* gval, void* gtarget, int B, int C, int Hi, int Wi, int H, int W, int ks, int dil, double eps, int dtype,
                        int accumulate, cudaStream_t st_) {
     if (gin1 != nullptr && !accumulate) {
-        const int e = zero_async(gin1, (size_t)B * C * Hi * Wi * elem_size(dtype), st_);
+        const int e = zero_async(gin1, (size_t)B * C * Hi * Wi * rs_gin1_bytes(dtype), st_);
         if (e != GFLA_OK) return e;
     }
-    if (dtype == GFLA_F32) { GFLA_RS_DISPATCH(float, rs_launch_cos_bwd, in1, in2, target, stats, gcos, gin1, gin2, gval, gtarget, B, C, Hi, Wi, H, W, dil, eps, accumulate, st_) }
-    if (dtype == GFLA_F64) { GFLA_RS_DISPATCH(double, rs_launch_cos_bwd, in1, in2, target, stats, gcos, gin1, gin2, gval, gtarget, B, C, Hi, Wi, H, W, dil, eps, accumulate, st_) }
-    return GFLA_E_DTYPE;
+    GFLA_RS_DTYPES(dtype, rs_launch_cos_bwd, in1, in2, target, stats, gcos, gin1, gin2, gval, gtarget, B, C, Hi, Wi, H, W, dil, eps, accumulate, st_)
 }
 
 }  // namespace gfla

@@ -48,6 +48,20 @@ def _stream(t: torch.Tensor) -> int:
     return torch.cuda.current_stream(t.device).cuda_stream
 
 
+_HALF = (torch.bfloat16, torch.float16)
+
+
+def flow_f32(data: torch.Tensor, flow: torch.Tensor) -> torch.Tensor:
+    """The flow a warping op runs with, given the dtype of the feature maps it warps.  16-bit feature maps pair with an
+    fp32 flow: the tap positions and fractions are then decided in fp32, bit-identical to the fp32 kernels (and the
+    tensor-core tile kernels take an fp32 flow only).  A 16-bit flow next to fp32 feature maps (a bf16 generator feeding
+    an fp32 VGG) is widened as well.  Any other pairing is returned as is.  autograd casts the flow's gradient back to
+    the flow's own dtype."""
+    if flow.dtype != torch.float32 and (data.dtype in _HALF or (data.dtype == torch.float32 and flow.dtype in _HALF)):
+        return flow.float()
+    return flow
+
+
 def _p(t):
     return None if t is None else t.data_ptr()
 
@@ -211,22 +225,39 @@ def resample2d_fwd(input1: torch.Tensor, input2: torch.Tensor, kernel_size: int,
     _, d, hi, wi = input1.size()
     b, three, h, w = input2.size()
     assert three == 3, "input2 must be [B,3,H,W] = (dx, dy, sigma) (resample2d.py:51-52)"
-    if input2.dtype != input1.dtype:
+    input2 = flow_f32(input1, input2)
+    half = input1.dtype in _HALF
+    if not half and input2.dtype != input1.dtype:
         raise TypeError("resample2d: input1 and input2 must share a dtype (float32 or float64)")
     out = input1.new_empty((b, d, h, w))
+    fn = _lib.lib().gfla_resample2d16_fwd if half else _lib.lib().gfla_resample2d_fwd
     with torch.cuda.device_of(input1):
-        _lib.check(_lib.lib().gfla_resample2d_fwd(_p(input1), _p(input2), _p(out), b, d, hi, wi, h, w, kernel_size,
-                                                  dilation, _dt(input1), _stream(input1)), "resample2d_fwd")
+        _lib.check(fn(_p(input1), _p(input2), _p(out), b, d, hi, wi, h, w, kernel_size, dilation, _dt(input1), _stream(input1)),
+                   "resample2d_fwd")
     return out
 
 
 def resample2d_bwd(input1, input2, grad_out, kernel_size, dilation, grad_input1=None, grad_input2=None):
+    """-> (grad_input1, grad_input2).  If buffers are passed (fp32 / fp64 only), the gradients are ADDED into them.  16-bit
+    input1: grad_input1 in input1's dtype (summed in an fp32 buffer and rounded once), grad_input2 in fp32."""
     alert_not_deterministic("resample2d backward (grad_input1 scatter)")
     assert input1.is_contiguous() and input2.is_contiguous()
     grad_out = grad_out.contiguous()
     _need_cuda(input1, input2, grad_out)
     _, d, hi, wi = input1.size()
     b, _, h, w = input2.size()
+    input2 = flow_f32(input1, input2)
+    if input1.dtype in _HALF:
+        if grad_input1 is not None or grad_input2 is not None:
+            raise TypeError("resample2d backward of 16-bit input1: the gradients are returned, not added into buffers")
+        if grad_out.dtype != input1.dtype:
+            raise TypeError(f"resample2d backward: grad_out must have input1's dtype {input1.dtype}, got {grad_out.dtype}")
+        gin1 = torch.empty(input1.shape, dtype=torch.float32, device=input1.device)
+        gin2 = torch.empty_like(input2)
+        with torch.cuda.device_of(input1):
+            _lib.check(_lib.lib().gfla_resample2d16_bwd(_p(input1), _p(input2), _p(grad_out), _p(gin1), _p(gin2), b, d, hi, wi, h, w,
+                                                        kernel_size, dilation, _dt(input1), 0, _stream(input1)), "resample2d_bwd")
+        return convert(gin1, input1.dtype), gin2
     accumulate = 1
     if grad_input1 is None:
         grad_input1, grad_input2, accumulate = torch.empty_like(input1), torch.empty_like(input2), 0
@@ -239,42 +270,57 @@ def resample2d_bwd(input1, input2, grad_out, kernel_size, dilation, grad_input1=
 
 def resample2d_cosine_fwd(input1, input2, target, kernel_size: int, dilation: int, eps: float = 1e-8):
     """cos[b,y,x] = cosine_similarity(resample2d(input1, input2)[b,:,y,x], target[b,:,y,x]) without the warped tensor
-    (external_function.py:275-279).  -> (cos [B,H,W], stats [B,3,H,W] for the backward)"""
+    (external_function.py:275-279).  -> (cos [B,H,W], stats [B,3,H,W] for the backward).  16-bit input1 and target: cos in
+    their dtype, stats in fp32."""
     assert input1.is_contiguous() and input2.is_contiguous() and target.is_contiguous()
     _need_cuda(input1, input2, target)
     _, d, hi, wi = input1.size()
     b, three, h, w = input2.size()
     assert three == 3, "input2 must be [B,3,H,W] = (dx, dy, sigma) (resample2d.py:51-52)"
     assert tuple(target.shape) == (b, d, h, w), "target must be [B,C,H,W] on the flow's grid"
-    if input2.dtype != input1.dtype or target.dtype != input1.dtype:
-        raise TypeError("resample2d_cosine: input1, input2 and target must share a dtype (float32 or float64)")
+    input2 = flow_f32(input1, input2)
+    half = input1.dtype in _HALF
+    if (not half and input2.dtype != input1.dtype) or target.dtype != input1.dtype:
+        raise TypeError("resample2d_cosine: input1, input2 and target must share a dtype (float32 or float64), or input1 and "
+                        "target a 16-bit one")
     cos = input1.new_empty((b, h, w))
-    stats = input1.new_empty((b, 3, h, w))
+    stats = input2.new_empty((b, 3, h, w))
+    fn = _lib.lib().gfla_resample2d16_cosine_fwd if half else _lib.lib().gfla_resample2d_cosine_fwd
     with torch.cuda.device_of(input1):
-        _lib.check(_lib.lib().gfla_resample2d_cosine_fwd(_p(input1), _p(input2), _p(target), _p(cos), _p(stats), b, d, hi, wi, h, w,
-                                                         kernel_size, dilation, float(eps), _dt(input1), _stream(input1)),
-                   "resample2d_cosine_fwd")
+        _lib.check(fn(_p(input1), _p(input2), _p(target), _p(cos), _p(stats), b, d, hi, wi, h, w, kernel_size, dilation, float(eps),
+                      _dt(input1), _stream(input1)), "resample2d_cosine_fwd")
     return cos, stats
 
 
 def resample2d_cosine_bwd(input1, input2, target, stats, grad_cos, kernel_size, dilation, eps=1e-8, need_input1=False,
                           need_target=False):
-    """-> (grad_input1 | None, grad_input2, grad_target | None)"""
+    """-> (grad_input1 | None, grad_input2, grad_target | None).  16-bit input1: grad_input1 summed in an fp32 buffer and
+    rounded once to input1's dtype, grad_input2 in fp32, grad_target in the target's dtype."""
     if need_input1:
         alert_not_deterministic("resample2d_cosine backward (grad_input1 scatter)")
     grad_cos = grad_cos.contiguous()
     _need_cuda(input1, input2, target, stats, grad_cos)
     _, d, hi, wi = input1.size()
     b, _, h, w = input2.size()
+    input2 = flow_f32(input1, input2)
+    half = input1.dtype in _HALF
+    if half and (grad_cos.dtype != input1.dtype or stats.dtype != torch.float32):
+        raise TypeError(f"resample2d_cosine backward: grad_cos must be {input1.dtype} and stats float32, got {grad_cos.dtype} / "
+                        f"{stats.dtype}")
+    wide = torch.float32 if half else input1.dtype                 # grad_input1 and its grad_val scratch
     grad_in2 = torch.empty_like(input2)
-    grad_in1 = torch.empty_like(input1) if need_input1 else None
-    grad_val = torch.empty_like(target) if need_input1 else None
+    grad_in1 = torch.empty_like(input1, dtype=wide) if need_input1 else None
+    grad_val = torch.empty_like(target, dtype=wide) if need_input1 else None
     grad_target = torch.empty_like(target) if need_target else None
+    fn = _lib.lib().gfla_resample2d16_cosine_bwd if half else _lib.lib().gfla_resample2d_cosine_bwd
     with torch.cuda.device_of(input1):
-        _lib.check(_lib.lib().gfla_resample2d_cosine_bwd(
+        _lib.check(fn(
             _p(input1), _p(input2), _p(target), _p(stats), _p(grad_cos), _p(grad_in1) if need_input1 else None, _p(grad_in2),
             _p(grad_val) if need_input1 else None, _p(grad_target) if need_target else None, b, d, hi, wi, h, w, kernel_size, dilation,
             float(eps), _dt(input1), 0, _stream(input1)), "resample2d_cosine_bwd")
+    if half and need_input1:
+        del grad_val
+        grad_in1 = convert(grad_in1, input1.dtype)
     return grad_in1, grad_in2, grad_target
 
 

@@ -22,7 +22,7 @@ class Resample2dFunction(Function):
     def backward(ctx, grad_output):
         input1, input2 = ctx.saved_tensors
         grad_input1, grad_input2 = F_.resample2d_bwd(input1, input2, grad_output, ctx.kernel_size, ctx.dilation)
-        return grad_input1, grad_input2, None, None
+        return grad_input1, grad_input2.to(input2.dtype), None, None
 
 
 class Resample2d(Module):
@@ -31,7 +31,10 @@ class Resample2d(Module):
     One deliberate difference: the reference builds ``self.sigma`` with
     ``.cuda()`` inside ``__init__`` (resample2d.py:47), which needs a GPU at
     construction time and pins the module to device 0; here sigma is kept as a
-    Python float and materialised on the input's device in ``forward``."""
+    Python float and materialised on the input's device in ``forward``.
+
+    bf16 / fp16 ``input1`` runs on the 16-bit kernels with an fp32 flow (a 16-bit flow is widened, and so is one next
+    to an fp32 ``input1``): the output has ``input1``'s dtype, each gradient the dtype of its own input."""
 
     def __init__(self, kernel_size=2, dilation=1, sigma=5):
         super(Resample2d, self).__init__()
@@ -41,6 +44,7 @@ class Resample2d(Module):
 
     def forward(self, input1, input2):
         input1_c = input1.contiguous()
+        input2 = F_.flow_f32(input1_c, input2)            # the sigma plane is built in the dtype the kernels read
         sigma = torch.full((input2.size(0), 1, input2.size(2), input2.size(3)), self.sigma,
                            dtype=input2.dtype, device=input2.device)
         input2 = torch.cat((input2, sigma), 1)
@@ -68,7 +72,7 @@ class Resample2dCosineFunction(Function):
         ks, dil, eps = ctx.cfg
         g1, g2, gt = F_.resample2d_cosine_bwd(input1, input2, target, stats, grad_cos, ks, dil, eps,
                                               need_input1=ctx.needs_input_grad[0], need_target=ctx.needs_input_grad[2])
-        return g1, g2, gt, None, None, None
+        return g1, g2.to(input2.dtype), gt, None, None, None
 
 
 class Resample2dCosine(Module):
@@ -83,6 +87,7 @@ class Resample2dCosine(Module):
         self.eps = float(eps)
 
     def forward(self, input1, input2, target):
+        input2 = F_.flow_f32(input1, input2)
         sigma = torch.full((input2.size(0), 1, input2.size(2), input2.size(3)), self.sigma, dtype=input2.dtype, device=input2.device)
         input2 = torch.cat((input2, sigma), 1)
         return Resample2dCosineFunction.apply(input1.contiguous(), input2, target, self.kernel_size, self.dilation, self.eps)

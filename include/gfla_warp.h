@@ -136,7 +136,8 @@ int gfla_attn_reshape_bwd(const void* grad_out, void* grad_in, int B, int H, int
  *   in1 [B,C,Hi,Wi]; in2 [B,3,H,W] = (dx, dy, sigma) -- the sigma plane is
  *   appended by the Python module (resample2d.py:51-52); out [B,C,H,W];
  *   grad_in2 [B,3,H,W] (all three planes are written, like :328).
- *   in2 / grad_in2 have the same dtype as in1 (F32 or F64 only).
+ *   in2 / grad_in2 have the same dtype as in1 (F32 or F64 only; 16-bit
+ *   feature maps: gfla_resample2d16_*, below).
  * ------------------------------------------------------------------------ */
 int gfla_resample2d_fwd(const void* in1, const void* in2, void* out,
                         int B, int C, int Hi, int Wi, int H, int W, int ks, int dilation,
@@ -173,6 +174,36 @@ int gfla_resample2d_cosine_bwd(const void* in1, const void* in2, const void* tar
                                void* grad_in1, void* grad_in2, void* grad_val, void* grad_target,
                                int B, int C, int Hi, int Wi, int H, int W, int ks, int dilation,
                                double eps, int dtype, int accumulate, gfla_stream_t stream);
+
+/* ------------------------------------------------------------------------ *
+ * resample2d and resample2d -> cosine on 16-bit feature maps
+ *   Same operations, shapes and arguments as the four entry points above, for
+ *   dtype = GFLA_BF16 or GFLA_F16 (anything else: GFLA_E_DTYPE).
+ *   In dtype: in1, out, grad_out, target, cos_out, grad_cos, grad_target.
+ *   In fp32: in2 (dx, dy, sigma), grad_in2, stats, grad_in1 and grad_val.
+ *   A call computes exactly what the F32 entry point computes on the widened
+ *   16-bit inputs (the taps are decided in fp32, all arithmetic is fp32) and
+ *   rounds each dtype output once, at its store.  grad_in1 is scattered with
+ *   fp32 atomics into the fp32 buffer, as in the F32 call (no 16-bit atomics);
+ *   the caller narrows it once, e.g. with gfla_convert.  With accumulate = 1 a
+ *   dtype grad_target is widened, added to in fp32 and rounded once.
+ * ------------------------------------------------------------------------ */
+int gfla_resample2d16_fwd(const void* in1, const void* in2_f32, void* out,
+                          int B, int C, int Hi, int Wi, int H, int W, int ks, int dilation,
+                          int dtype, gfla_stream_t stream);
+int gfla_resample2d16_bwd(const void* in1, const void* in2_f32, const void* grad_out,
+                          void* grad_in1_f32, void* grad_in2_f32,
+                          int B, int C, int Hi, int Wi, int H, int W, int ks, int dilation,
+                          int dtype, int accumulate, gfla_stream_t stream);
+int gfla_resample2d16_cosine_fwd(const void* in1, const void* in2_f32, const void* target,
+                                 void* cos_out, void* stats_f32,
+                                 int B, int C, int Hi, int Wi, int H, int W, int ks, int dilation,
+                                 double eps, int dtype, gfla_stream_t stream);
+int gfla_resample2d16_cosine_bwd(const void* in1, const void* in2_f32, const void* target,
+                                 const void* stats_f32, const void* grad_cos,
+                                 void* grad_in1_f32, void* grad_in2_f32, void* grad_val_f32, void* grad_target,
+                                 int B, int C, int Hi, int Wi, int H, int W, int ks, int dilation,
+                                 double eps, int dtype, int accumulate, gfla_stream_t stream);
 
 /* ------------------------------------------------------------------------ *
  * fused local attention = the tail of ExtractorAttn.forward

@@ -224,3 +224,123 @@ if "module" in which:   # ExtractorAttn at the shapes the pose generator uses (S
             fb = timed(lambda: fn(True), n=3, w=2)
             print(json.dumps({"op": name, "config": f"B={B} C={C} {HW}x{HW} k={k} bf16 channels_last", "fwd_ms": round(f, 4),
                               "fwd_bwd_ms": round(fb, 4), "Mpixels_per_s_fwd_bwd": round(px / fb / 1e3, 2)}), flush=True)
+
+if "resample16" in which:   # resample2d and the fused resample2d -> cosine on bf16 feature maps: three arms alternated in one process
+    # (a) bf16 on the 16-bit kernels; (b) fp32 data on the fp32 kernels; (c) bf16 -> .float() -> fp32 kernels -> .to(bf16)
+    import statistics
+    import subprocess
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+    card = q.stdout.strip() or torch.cuda.get_device_name(0)
+    bf = torch.bfloat16
+
+    def arms3(name, px, fns, alg, cfg, rounds=5, **kw):
+        """fns: {arm: fn}; alg: {arm: algorithmic bytes}; median of `rounds` alternated rounds per arm"""
+        t = {a: [] for a in fns}
+        for _ in range(rounds):
+            for a, fn in fns.items():
+                t[a].append(timed(fn, n=3, w=1))
+        for a in fns:
+            emit(f"{name} ({a})", statistics.median(t[a]), px, alg[a], config=cfg, card=card, rounds=rounds, **kw)
+        return {a: statistics.median(v) for a, v in t.items()}
+
+    B, C, H, W = 32, 128, 512, 512           # cfg3
+    px = B * H * W
+    x32 = torch.randn(B, C, H, W, device=dev)
+    g32 = torch.randn(B, C, H, W, device=dev)
+    x16, g16 = x32.to(bf), g32.to(bf)
+    coarse = (torch.rand(B, 2, H // 16, W // 16, device=dev) * 16 - 8).floor() + 0.25
+    blocky = (torch.nn.functional.interpolate(coarse, size=(H, W), mode="nearest") + 0.5 * torch.rand(B, 2, H, W, device=dev)).contiguous()
+    # the fp32 grad_in1 buffer of arm (a): zero fill (4 B), 4 B instead of 2 B per element, narrowing (read 4 B, write 2 B)
+    extra = px * C * 12
+    for ks, sigma in ((2, 5.0), (4, 2.0)):
+        for fname, fl in (("smooth", smooth(B, H, W)), ("blocky", blocky)):
+            in2 = torch.cat([fl, torch.full((B, 1, H, W), sigma, device=dev)], 1).contiguous()
+            fwd = {"a bf16": lambda: F_.resample2d_fwd(x16, in2, ks, 1),
+                   "b fp32": lambda: F_.resample2d_fwd(x32, in2, ks, 1),
+                   "c bf16 via fp32": lambda: F_.resample2d_fwd(x16.float(), in2, ks, 1).to(bf)}
+            arms3(f"resample2d_fwd ks={ks} {fname} flow", px, fwd,
+                  {"a bf16": px * (2 * C * 2 + 12), "b fp32": px * (2 * C * 4 + 12), "c bf16 via fp32": px * (2 * C * 2 + 12)},
+                  "cfg3 B=32 C=128 512x512")
+
+            def bwd_c():
+                g1, g2 = F_.resample2d_bwd(x16.float(), in2, g16.float(), ks, 1)
+                return g1.to(bf), g2
+            bwd = {"a bf16": lambda: F_.resample2d_bwd(x16, in2, g16, ks, 1),
+                   "b fp32": lambda: F_.resample2d_bwd(x32, in2, g32, ks, 1),
+                   "c bf16 via fp32": bwd_c}
+            arms3(f"resample2d_bwd ks={ks} {fname} flow", px, bwd,
+                  {"a bf16": px * (3 * C * 2 + 24), "b fp32": px * (3 * C * 4 + 24), "c bf16 via fp32": px * (3 * C * 2 + 24)},
+                  "cfg3", extra_impl_GB_arm_a=round(extra / 1e9, 3))
+            torch.cuda.empty_cache()
+    del x32, g32, x16, g16, blocky, coarse
+    torch.cuda.empty_cache()
+
+    for lname, (B, C, H, W) in (("relu3_1", (16, 256, 64, 64)), ("relu2_1", (16, 128, 128, 128))):   # bench.py's f4 shapes
+        px = B * H * W
+        s32, t32 = torch.randn(B, C, H, W, device=dev), torch.randn(B, C, H, W, device=dev)
+        s16, t16 = s32.to(bf), t32.to(bf)
+        in2 = torch.cat([smooth(B, H, W), torch.full((B, 1, H, W), 2.0, device=dev)], 1).contiguous()
+        gc32 = torch.randn(B, H, W, device=dev)
+        gc16 = gc32.to(bf)
+        st16 = F_.resample2d_cosine_fwd(s16, in2, t16, 4, 1)[1]
+        st32 = F_.resample2d_cosine_fwd(s32, in2, t32, 4, 1)[1]
+
+        def step_a():
+            c, st = F_.resample2d_cosine_fwd(s16, in2, t16, 4, 1)
+            F_.resample2d_cosine_bwd(s16, in2, t16, st, gc16, 4, 1)
+
+        def step_b():
+            c, st = F_.resample2d_cosine_fwd(s32, in2, t32, 4, 1)
+            F_.resample2d_cosine_bwd(s32, in2, t32, st, gc32, 4, 1)
+
+        def step_c():
+            a, t = s16.float(), t16.float()
+            c, st = F_.resample2d_cosine_fwd(a, in2, t, 4, 1)
+            c.to(bf)
+            F_.resample2d_cosine_bwd(a, in2, t, st, gc16.float(), 4, 1)
+
+        # forward: source, target, flow, cos, stats; flow-only backward: source, target, stats, grad_cos, flow, grad_flow
+        alg = {"a bf16": px * (4 * C + 2 + 12 + 12) + px * (4 * C + 12 + 2 + 12 + 12),
+               "b fp32": px * (8 * C + 4 + 12 + 12) + px * (8 * C + 12 + 4 + 12 + 12),
+               "c bf16 via fp32": px * (4 * C + 2 + 12 + 12) + px * (4 * C + 12 + 2 + 12 + 12)}
+        arms3(f"resample2d_cosine fwd+flow bwd {lname}", px, {"a bf16": step_a, "b fp32": step_b, "c bf16 via fp32": step_c}, alg,
+              f"f4 {lname} B={B} C={C} {H}x{W} ks=4 sigma=2")
+        del s32, t32, s16, t16
+        torch.cuda.empty_cache()
+
+    # peak memory of one PerceptualCorrectness forward + backward (random-weight VGG19, frozen) in bf16 and in fp32
+    import torchvision
+    import gfla_b200
+    torch.manual_seed(0)
+    feats = torchvision.models.vgg19(weights=None).features[:21].to(dev).eval()
+    for p in feats.parameters():
+        p.requires_grad_(False)
+    cuts = {"relu1_1": 1, "relu2_1": 6, "relu3_1": 11, "relu4_1": 20}
+
+    class VGG(torch.nn.Module):
+        def __init__(self, f):
+            super().__init__()
+            self.f = f
+
+        def forward(self, x):
+            out, h = {}, x
+            for i, layer in enumerate(self.f):
+                h = layer(h)
+                out.update({n: h for n, c in cuts.items() if c == i})
+            return out
+    for dt in (bf, torch.float32):
+        vgg = VGG(feats.to(dt))
+        imgs = [torch.rand(16, 3, 256, 256, device=dev).to(dt) for _ in range(2)]
+        flows = [(torch.rand(16, 2, h, h, device=dev) * 4 - 2).to(dt).requires_grad_() for h in (64, 128)]
+        loss_fn = gfla_b200.PerceptualCorrectness(vgg=vgg)
+        loss_fn(imgs[0], imgs[1], flows, [2, 1]).backward()          # warm-up
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        base = torch.cuda.memory_allocated()
+        loss_fn(imgs[0], imgs[1], flows, [2, 1]).backward()
+        torch.cuda.synchronize()
+        print(json.dumps({"op": "PerceptualCorrectness fwd+bwd peak memory", "dtype": str(dt), "card": card,
+                          "config": "VGG19 features to relu4_1, 16x3x256x256 images, flows at relu3_1 and relu2_1",
+                          "peak_extra_MB": round((torch.cuda.max_memory_allocated() - base) / 2 ** 20, 1)}), flush=True)
+        del vgg, imgs, flows, loss_fn
+        torch.cuda.empty_cache()
