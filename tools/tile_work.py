@@ -1,18 +1,24 @@
 """Host-side count of the work the tensor-core tile kernels do on the bench workload (cfg2: B=16, 256x256, k=5, C=256),
 with and without skipping the MMA tiles of inactive 16-pixel group rows.
 
-    python tools/tile_work.py [--flow smooth|iid|both] [--seed N] [--B 16] [--H 256] [--W 256] [--k 5]
+    python tools/tile_work.py [--flow smooth|iid|both] [--seed N] [--B 16] [--H 256] [--W 256] [--k 5] [--C 256] [--cn 128]
 
 Flows come from bench.py's two families (smooth = x16 bilinear up-sampling of U(-8,8), iid = U(-8,8)) drawn with their
 own seed, so these are statistics of the family, not of the bench's exact tensors.  The tap arithmetic is the kernels'
-(axis_tap in fp32, clamped windows), the footprint is group_bbox's and the steps are the kernels' row-major walk over
-16-position segments.  A pixel is active in a step when window_meets_step holds (tile_window.cuh); irregular pixels never are.
+(axis_tap in fp32, clamped windows), the footprint is group_bbox's and the steps are the kernels' row-major walk over the
+footprint.  A pixel is active in a K-step (16 positions) when window_meets_step holds (tile_window.cuh); irregular
+pixels never are.  Warps of 32 pixels, mma.sync m16n8k16, ldmatrix .x4 = 512 B.
 
-Per-CTA-step costs (C = 256, warps of 32 pixels, mma.sync m16n8k16, ldmatrix .x4 = 512 B):
-  forward   4 passes of 64 channels; per warp and pass: 2 A + 4 B ldmatrix, 16 MMAs; skip: an inactive m-tile drops its
-            A ldmatrix and 8 MMAs, a warp without active pixels drops everything
-  backward  1 pass of 256 channels; P GEMM per warp: 16 k-steps x (2 A + 1 B) ldmatrix, 4 MMAs; GS GEMM per group row:
-            4 warps x (1 + 4) ldmatrix, 4 x 8 MMAs; skip: inactive m-tiles / group rows drop theirs, a step without any drops all
+Channels-last forward (k_local_attn_fwd_tc_cl), counted per CTA over C / CN passes of CN channels and 32-position steps
+(two K-steps each):
+  MMAs      CN / 8 per m-tile (16 pixels) active in a K-step
+  ldmatrix  per K-step, 1 A per active m-tile, CN / 16 B per MMA warp with an active m-tile
+  slab      bytes stored into the weight slabs: the pixel warps' window entries (2 B each, scattered), the MMA warps'
+            zero fill (64 B per slab row of an m-tile active in either K-step of the step)
+  barriers  per step FULL and FREE (256 threads each)
+Backward, per CTA-step (16-position steps, one pass of 256 channels): P GEMM per warp: 16 k-steps x (2 A + 1 B)
+ldmatrix, 4 MMAs; GS GEMM per group row: 4 warps x (1 + 4) ldmatrix, 4 x 8 MMAs; skip: inactive m-tiles / group rows
+drop theirs, a step without any drops all.
 
 grad_source reductions of the backward, per CTA-step.  A position of the step receives a partial sum when some active
 pixel's clamped window covers it (every window entry is taken as nonzero).  Each warp adds its 64 channels of the
@@ -52,7 +58,7 @@ def taps(flow, coord, k, dim):
     return fl[0], regular, lo, hi
 
 
-def count(flow, k):
+def count(flow, k, C, CN):
     B, _, H, W = flow.shape
     ys, xs = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
     X0, rx, bxlo, bxhi = taps(flow[:, 0], xs[None], k, W)
@@ -62,7 +68,7 @@ def count(flow, k):
     cy0, cy1 = np.clip(Y0, 0, H - 1), np.clip(Y0 + k, 0, H - 1)
     inimg = np.ones((B, H, W), bool)
     st = dict(groups=0, steps=[], entries=0, rows_on=0, warps_on=0, empty=0,
-              f_mma=[0, 0], f_ldsm=[0, 0], b_mma=[0, 0], b_ldsm=[0, 0], red_ins=[0, 0], red_sec=[0, 0], f32_ins=0, f32_sec=0)
+              f_steps=0, f_mma=0, f_ldsm=0, f_scatter=0, f_zero=0, f_bar=0, b_mma=[0, 0], b_ldsm=[0, 0], red_ins=[0, 0], red_sec=[0, 0], f32_ins=0, f32_sec=0)
     for b in range(B):
         for gy in range(0, H, GH):
             for gx in range(0, W, GW):
@@ -87,12 +93,22 @@ def count(flow, k):
                 st["rows_on"] += nr.sum()
                 st["warps_on"] += rows.reshape(n, 4, 2).any(axis=2).sum()
                 st["empty"] += (nr == 0).sum()
-                # forward, 4 passes x 4 warps
-                st["f_mma"][0] += 4 * n * 4 * 16
-                st["f_ldsm"][0] += 4 * n * 4 * 6 * LDSM
                 wtiles = rows.reshape(n, 4, 2)
-                st["f_mma"][1] += 4 * 8 * wtiles.sum()
-                st["f_ldsm"][1] += 4 * (wtiles.sum() + 4 * wtiles.any(axis=2).sum()) * LDSM
+                # forward: 32-position steps, K-steps x and x + 16, C / CN passes that repeat the same walk
+                passes = C // CN
+                hx = np.arange(bx0, bx1 + 1, 2 * SEG)
+                n2 = len(sy) * len(hx)
+                y2 = np.repeat(sy, len(hx))[:, None, None]
+                x2 = np.tile(hx, len(sy))[:, None, None] + np.array([0, SEG])[None, :, None]       # [steps, 2, 1]
+                act2 = reg[None, None] & (a_y0[None] <= y2) & (y2 <= a_y1[None]) & (a_x0[None] < x2 + SEG) & (a_x1[None] >= x2)
+                ent2 = (np.clip(np.minimum(a_x1[None], x2 + SEG - 1) - np.maximum(a_x0[None], x2) + 1, 0, None) * act2).sum()
+                tiles2 = act2.reshape(n2, 2, 8, 16).any(axis=3)                                 # [steps, K-steps, m-tiles]
+                st["f_steps"] += passes * n2
+                st["f_mma"] += passes * (CN // 8) * tiles2.sum()
+                st["f_ldsm"] += passes * (tiles2.sum() + (CN // 16) * tiles2.reshape(n2, 2, 4, 2).any(axis=3).sum()) * LDSM
+                st["f_scatter"] += passes * 2 * ent2
+                st["f_zero"] += passes * 16 * 2 * (2 * SEG) * tiles2.any(axis=1).sum()
+                st["f_bar"] += passes * 2 * n2
                 # backward, one pass of 256 channels
                 st["b_mma"][0] += n * (4 * 16 * 4 + 8 * 32)
                 st["b_ldsm"][0] += n * (4 * 16 * 3 + 8 * 20) * LDSM
@@ -123,7 +139,12 @@ def report(kind, st):
     print(f"active 16-pixel group rows          {100 * st['rows_on'] / (n * 8):.1f} %")
     print(f"active warps (32 pixels)            {100 * st['warps_on'] / (n * 4):.1f} %")
     print(f"steps without any active pixel      {100 * st['empty'] / n:.1f} %")
-    for name, m, l in (("forward", st["f_mma"], st["f_ldsm"]), ("backward", st["b_mma"], st["b_ldsm"])):
+    g = st["groups"]
+    print(f"forward per CTA ({st['C']} channels in passes of {st['CN']}): {st['f_steps'] / g:.1f} steps, {st['f_mma'] / g:.0f} MMAs, "
+          f"ldmatrix {st['f_ldsm'] / g / 1024:.1f} KB, slab stores {st['f_scatter'] / g / 1024:.1f} KB scattered + "
+          f"{st['f_zero'] / g / 1024:.1f} KB zero fill, {st['f_bar'] / g:.0f} barriers")
+    print(f"forward per CTA-step: {st['f_mma'] / st['f_steps']:.1f} MMAs, ldmatrix {st['f_ldsm'] / st['f_steps'] / 1024:.1f} KB")
+    for name, m, l in (("backward", st["b_mma"], st["b_ldsm"]),):
         print(f"{name:9s} per CTA-step   MMAs {m[0] / n:7.1f} -> {m[1] / n:7.1f}   ldmatrix {l[0] / n / 1024:6.1f} KB -> {l[1] / n / 1024:6.1f} KB"
               f"   ({100 * (1 - m[1] / m[0]):.0f} % / {100 * (1 - l[1] / l[0]):.0f} % skipped)")
     ri, rs = st["red_ins"], st["red_sec"]
@@ -140,9 +161,13 @@ def main():
     ap.add_argument("--H", type=int, default=256)
     ap.add_argument("--W", type=int, default=256)
     ap.add_argument("--k", type=int, default=5)
+    ap.add_argument("--C", type=int, default=256)
+    ap.add_argument("--cn", type=int, default=128, choices=[64, 128], help="channels per forward pass")
     a = ap.parse_args()
     for kind in (["smooth", "iid"] if a.flow == "both" else [a.flow]):
-        report(kind, count(make_flow(kind, a.B, a.H, a.W, a.seed), a.k))
+        st = count(make_flow(kind, a.B, a.H, a.W, a.seed), a.k, a.C, a.cn)
+        st.update(C=a.C, CN=a.cn)
+        report(kind, st)
 
 
 if __name__ == "__main__":
