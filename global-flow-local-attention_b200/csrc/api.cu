@@ -16,7 +16,7 @@ int resample2d_cos_bwd(const void*, const void*, const void*, const void*, const
 int local_attn_fwd_gather(const void*, const void*, const void*, void*, void*, const void*, const void*, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
 int local_attn_bwd_gather(const void*, const void*, const void*, const void*, void*, void*, void*, int, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
 bool local_attn_bwd_tc_supported(int C, int k, int dtype, int flow_dtype, int layout, const void* src, const void* gout, const void* gsrc);
-int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow, void* glogits, int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate, cudaStream_t);
+int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow, void* glogits, int B, int C, int Hs, int Ws, int H, int W, int k, int dtype, int accumulate, cudaStream_t);
 int local_attn_fwd_tc(const void*, const void*, const void*, void*, void*, const void*, const void*, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
 int relayout(const void*, void*, int, int, int, int, int, int, cudaStream_t);
 bool local_attn_fwd_tc_supported(int C, int Ws, int k, int dtype, int flow_dtype, int layout, const void* src, const void* out);
@@ -26,8 +26,8 @@ int patch_conv_bwd(const void*, const void*, const void*, const void*, void*, vo
                    cudaStream_t);
 int local_attn_bwd_gather_det(const void*, const void*, const void*, const void*, void*, void*, int, int, int, int, int, int, int, int, int,
                               int, int, fx_t*, const int*, cudaStream_t);
-int local_attn_bwd_tc_det(const void*, const void*, const void*, const void*, void*, void*, int, int, int, int, int, int, int, int, fx_t*,
-                          const int*, cudaStream_t);
+int local_attn_bwd_tc_det(const void*, const void*, const void*, const void*, void*, void*, int, int, int, int, int, int, int, int, int,
+                          fx_t*, const int*, cudaStream_t);
 int block_extract_bwd_det(const void*, const void*, const void*, void*, int, int, int, int, int, int, int, int, int, int, fx_t*, const int*,
                           cudaStream_t);
 int patch_conv_bwd_det(const void*, const void*, const void*, const void*, void*, int, int, int, int, int, int, int, int, fx_t*, fx_t*,
@@ -282,8 +282,8 @@ int gfla_local_attn_bwd(const void* source, const void* flow, const void* logits
     const bool tc_ok = local_attn_bwd_tc_supported(C, k, dtype, flow_dtype, layout, source, grad_out, grad_source);
     if (algo == 2 && !tc_ok) return GFLA_E_NOTSUP;
     if (algo == 2 || (algo == 0 && tc_ok))
-        return local_attn_bwd_tc(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, accumulate,
-                                 (cudaStream_t)stream);
+        return local_attn_bwd_tc(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype,
+                                 accumulate, (cudaStream_t)stream);
     return local_attn_bwd_gather(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W,
                                  k, dtype, flow_dtype, accumulate, layout, (cudaStream_t)stream);
 }
@@ -372,12 +372,16 @@ int gfla_local_attn_bwd_det(const void* source, const void* flow, const void* lo
     // Bound of image b: every pixel spreads g_c times weights that sum to exactly 1/k^2 (softmax probabilities summing to
     // 1, times bilinear weights summing to 1, times 1/k^2) over the source positions, so every grad_source element of the
     // image is at most (H W / k^2) max|G_b| in magnitude, and so is the sum of the magnitudes of its partials.  The tile
-    // kernel rounds the weights to bf16 first: a factor of at most 1 + 2^-8, inside the margin (det_accum.cuh).
+    // kernel rounds the weights to the data's 16-bit type first.  bf16: a factor of at most 1 + 2^-8 on a pixel's weight
+    // sum.  fp16: a normal weight grows by at most 2^-11 of itself (factor 1 + 2^-11), and a weight below 2^-14 is
+    // subnormal and off by at most 2^-25 absolutely, (k+1)^2 2^-25 per pixel at most: against the pixel's weight sum 1/k^2
+    // that is k^2 (k+1)^2 2^-25 <= 900 2^-25 < 2^-15 (k <= 5, the only tile sizes).  Together below 1 + 2^-10.  Either
+    // factor stays far inside the one bit of margin below 2^62 (det_accum.cuh), which only requires a factor below 2.
     if (r == GFLA_OK) r = fx_exponents(amax, B, nullptr, (double)H * W / ((double)k * k), false, exps, st_);
     if (r == GFLA_OK) {
         if (algo == 2 || (algo == 0 && tc_ok))
-            r = local_attn_bwd_tc_det(source, flow, logits, grad_out, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, accumulate, sums,
-                                      exps, st_);
+            r = local_attn_bwd_tc_det(source, flow, logits, grad_out, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype, accumulate,
+                                      sums, exps, st_);
         else
             r = local_attn_bwd_gather_det(source, flow, logits, grad_out, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype,
                                           flow_dtype, accumulate, layout, sums, exps, st_);

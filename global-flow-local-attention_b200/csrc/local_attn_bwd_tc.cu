@@ -1,12 +1,13 @@
-// Fused local-attention backward on the tensor cores (channels-last bf16, fp32 flow, k in {3, 5}): ONE kernel for
-// grad_source, grad_flow and grad_logits.
+// Fused local-attention backward on the tensor cores (channels-last bf16 or fp16, fp32 flow, k in {3, 5}): ONE kernel for
+// grad_source, grad_flow and grad_logits.  T, the data's 16-bit type, is also the type of the weight slab and of the
+// grad_source partials; P stays fp32 in shared memory.
 //
 // Per 16x8 pixel group and 16-position row segment of the group's tap footprint (channels in passes of CN):
 //   * P[128 px][16 pos] = G[128 px][CN] * S[16 pos][CN]^T    the grad_out . source dot products of every pixel with
 //     every position of the segment; each pixel thread then picks its (k+1)^2 window entries out of P into Q (registers).
 //     Q is exactly the CUDA-core kernel's Q (local_attn.cu), so grad_flow / grad_logits follow from it per pixel with
 //     the same formulas (local_attn_pixel.cuh);
-//   * GS[16 pos][CN] = Wfull^T[16 pos][128 px] * G[128 px][CN] grad_source of the segment, added with 16-byte bf16
+//   * GS[16 pos][CN] = Wfull^T[16 pos][128 px] * G[128 px][CN] grad_source of the segment, added with 16-byte T
 //     reductions (the caller's buffer is zero-filled first unless the call accumulates).  Border positions, where the
 //     windows folded onto the image edge pile up, are summed in an fp32 scratch instead and rounded once (k_fold_border).
 // The grad_out tile G stays in shared memory for the whole pass; the source segment arrives by cp.async one step ahead.
@@ -54,9 +55,13 @@ struct BwdSmem {
     static constexpr int ALLOC = ROWS + BT_NAW * 4;
 };
 
-// 16-byte reduction: 8 bf16 values added element-wise, each add rounded once
-__device__ __forceinline__ void red_add_bf16x8(__nv_bfloat16* p, const uint32_t (&v)[4]) {
+// 16-byte reduction: 8 T values added element-wise, each add rounded once (fp16: a sum beyond 65504 becomes Inf)
+__device__ __forceinline__ void red_add_16x8(__nv_bfloat16* p, const uint32_t (&v)[4]) {
     asm volatile("red.global.add.noftz.v4.bf16x2 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
+                 : "memory");
+}
+__device__ __forceinline__ void red_add_16x8(__half* p, const uint32_t (&v)[4]) {
+    asm volatile("red.global.add.noftz.v4.f16x2 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
                  : "memory");
 }
 
@@ -73,7 +78,7 @@ __device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int t) {
 }
 
 // P GEMM of one warp for one step: the m-tiles whose pixel row is active (M0, M1) of its 32 pixels x 16 positions
-template <int CN, bool M0, bool M1>
+template <typename T, int CN, bool M0, bool M1>
 __device__ __forceinline__ void p_gemm(uint32_t ga, uint32_t sf, float (&pacc)[2][2][4]) {
     constexpr int GSTR = BwdSmem<CN>::GSTR;
 #pragma unroll 4
@@ -83,19 +88,19 @@ __device__ __forceinline__ void p_gemm(uint32_t ga, uint32_t sf, float (&pacc)[2
         if (M1) ldsm_x4(ga + 16 * GSTR + kk * 32, a1);
         ldsm_x4(sf + kk * 32, bf);
         if (M0) {
-            mma_bf16(pacc[0][0], a0, bf[0], bf[1]);
-            mma_bf16(pacc[0][1], a0, bf[2], bf[3]);
+            mma16<T>(pacc[0][0], a0, bf[0], bf[1]);
+            mma16<T>(pacc[0][1], a0, bf[2], bf[3]);
         }
         if (M1) {
-            mma_bf16(pacc[1][0], a1, bf[0], bf[1]);
-            mma_bf16(pacc[1][1], a1, bf[2], bf[3]);
+            mma16<T>(pacc[1][0], a1, bf[0], bf[1]);
+            mma16<T>(pacc[1][1], a1, bf[2], bf[3]);
         }
     }
 }
 
 // Slot of source position (y, x) on the image border (rows 0 and Hs-1, then columns 0 and Ws-1 of the rows between), in
 // [0, 2 (Hs + Ws)); -1 inside the image.  Windows folded onto the edge make border positions collect a share of nearly
-// every group of a border-clamped flow, and one bf16 atomic add per group would round each time.  Their grad_source is
+// every group of a border-clamped flow, and one 16-bit atomic add per group would round each time.  Their grad_source is
 // summed in an fp32 buffer instead and rounded once by k_fold_border.
 __device__ __forceinline__ int border_slot(int y, int x, int Hs, int Ws) {
     if (y == 0) return x;
@@ -108,8 +113,8 @@ __device__ __forceinline__ int border_slot(int y, int x, int Hs, int Ws) {
 // grad_out tile of the group for channels [c0, c0 + CN) into G, loaded by both warpgroups (pixels outside the image:
 // zeros).  Not fully unrolled: the compiler would then keep all the pass-invariant 64-bit addresses live across the step
 // loop, and at CN = 256 that spills.
-template <int CN>
-__device__ __forceinline__ void load_g_tile(uint32_t g_base, const __nv_bfloat16* __restrict__ go_b, int c0, int C, int gx0, int gy0,
+template <typename T, int CN>
+__device__ __forceinline__ void load_g_tile(uint32_t g_base, const T* __restrict__ go_b, int c0, int C, int gx0, int gy0,
                                             int H, int W, int tid) {
     constexpr int GSTR = BwdSmem<CN>::GSTR;
 #pragma unroll 4
@@ -122,25 +127,24 @@ __device__ __forceinline__ void load_g_tile(uint32_t g_base, const __nv_bfloat16
     cp_async_commit();
 }
 
-template <int K, bool DET>
-__device__ __forceinline__ void irregular_pixel_bwd(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow,
-                                                    const __nv_bfloat16* __restrict__ logits, const __nv_bfloat16* __restrict__ gout,
-                                                    __nv_bfloat16* __restrict__ gsrc, float* __restrict__ gflow,
-                                                    __nv_bfloat16* __restrict__ glogits, int b, int C, int Hs, int Ws, int H, int W,
+template <typename T, int K, bool DET>
+__device__ __forceinline__ void irregular_pixel_bwd(const T* __restrict__ src, const float* __restrict__ flow, const T* __restrict__ logits,
+                                                    const T* __restrict__ gout, T* __restrict__ gsrc, float* __restrict__ gflow,
+                                                    T* __restrict__ glogits, int b, int C, int Hs, int Ws, int H, int W,
                                                     int qx, int qy, int accumulate, int lane, fx_t* __restrict__ gsum,
                                                     double2 fsc) {
     constexpr int KK = K * K;
     const long long hw = (long long)H * W, qofs = (long long)qy * W + qx;
     const float fx = flow[(long long)b * 2 * hw + qofs], fy = flow[(long long)b * 2 * hw + hw + qofs];
     float p[KK], dp[KK];
-    pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + qofs, hw, KK, p);
+    pixel_softmax<T, float, KK>(logits + (long long)b * KK * hw + qofs, hw, KK, p);
     const float inv_kk = 1.0f / static_cast<float>(KK);
-    const __nv_bfloat16* s = src + (long long)b * Hs * Ws * C;
-    using GS = std::conditional_t<DET, fx_t, __nv_bfloat16>;
+    const T* s = src + (long long)b * Hs * Ws * C;
+    using GS = std::conditional_t<DET, fx_t, T>;
     GS* gs;
     if constexpr (DET) gs = gsum + (long long)b * Hs * Ws * C;
     else gs = gsrc + (long long)b * Hs * Ws * C;
-    const __nv_bfloat16* go = gout + ((long long)b * hw + qofs) * C;
+    const T* go = gout + ((long long)b * hw + qofs) * C;
     float gfx = 0.f, gfy = 0.f;
 #pragma unroll
     for (int i = 0; i < K; ++i) {
@@ -153,11 +157,11 @@ __device__ __forceinline__ void irregular_pixel_bwd(const __nv_bfloat16* __restr
             const float pij = p[i * K + j] * inv_kk;
             float q[4] = {0.f, 0.f, 0.f, 0.f};
             for (int c = lane; c < C; c += 32) {
-                const float g = __bfloat162float(go[c]);
-                q[0] += g * __bfloat162float(s[oLT + c]);
-                q[1] += g * __bfloat162float(s[oRT + c]);
-                q[2] += g * __bfloat162float(s[oLB + c]);
-                q[3] += g * __bfloat162float(s[oRB + c]);
+                const float g = ld(go + c);
+                q[0] += g * ld(s + oLT + c);
+                q[1] += g * ld(s + oRT + c);
+                q[2] += g * ld(s + oLB + c);
+                q[3] += g * ld(s + oRB + c);
                 const float gp = g * pij;
                 scatter_add<DET>(gs + oLT + c, gp * (tx.wlo * ty.wlo), fsc);
                 scatter_add<DET>(gs + oRT + c, gp * (tx.whi * ty.wlo), fsc);
@@ -172,18 +176,18 @@ __device__ __forceinline__ void irregular_pixel_bwd(const __nv_bfloat16* __restr
         }
     }
     if (lane == 0)
-        store_pixel_grads<__nv_bfloat16, float, float, KK>(p, dp, KK, gfx, gfy, glogits + (long long)b * KK * hw + qofs,
-                                                           gflow + (long long)b * 2 * hw + qofs, hw, accumulate);
+        store_pixel_grads<T, float, float, KK>(p, dp, KK, gfx, gfy, glogits + (long long)b * KK * hw + qofs,
+                                               gflow + (long long)b * 2 * hw + qofs, hw, accumulate);
 }
 
 // DET: grad_source goes into the fixed-point sums gsum with the image's exponent fx_exp[b] (det_accum.cuh); gsrc and
-// gborder are unused.  Each quad regroups its fp32 values so that every u64 reduction instruction of a warp covers
+// gborder are unused.  T comes last (here and in the forward kernels), so an instance's name still begins with its
+// shape parameters, k_local_attn_bwd_tc<K, CN, DET, T>.  Each quad regroups its fp32 values so that every u64 reduction instruction of a warp covers
 // 8 positions x 32 contiguous bytes: whole sectors.
-template <int K, int CN, bool DET = false>
+template <int K, int CN, bool DET, typename T>
 __global__ void __launch_bounds__(BT_THREADS, 2)
-k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow, const __nv_bfloat16* __restrict__ logits,
-                    const __nv_bfloat16* __restrict__ gout, __nv_bfloat16* __restrict__ gsrc, float* __restrict__ gflow,
-                    __nv_bfloat16* __restrict__ glogits, float* __restrict__ gborder, int C, int Hs, int Ws, int H, int W, int gcols,
+k_local_attn_bwd_tc(const T* __restrict__ src, const float* __restrict__ flow, const T* __restrict__ logits, const T* __restrict__ gout,
+                    T* __restrict__ gsrc, float* __restrict__ gflow, T* __restrict__ glogits, float* __restrict__ gborder, int C, int Hs, int Ws, int H, int W, int gcols,
                     int grows, int accumulate, fx_t* __restrict__ gsum, const int* __restrict__ fx_exp) {
     constexpr int K1 = K + 1, KK = K * K;
     using L = BwdSmem<CN>;
@@ -211,7 +215,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
         group_decode(gcols, grows, b, gx0, gy0);
         group_bbox<K>(flow, b, gx0, gy0, H, W, Hs, Ws, lane, bx0, by0, bx1, by1);
         const long long hw = (long long)H * W;
-        const __nv_bfloat16* go_b = gout + (long long)b * hw * C;
+        const T* go_b = gout + (long long)b * hw * C;
         // ---- per pixel: softmax, taps, window (folded, for grad_source) and the unfolded window origin (for Q)
         const int px = gx0 + (tid & 15), py = gy0 + (tid >> 4);
         const bool valid = px < W && py < H;
@@ -224,25 +228,25 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
         bool regular = false;
         if (valid) {
             float p[KK];
-            pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
+            pixel_softmax<T, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
             AxisTap<float> tx[K], ty[K];
             regular = taps_regular<float, K>(flow[(long long)b * 2 * hw + pofs], flow[(long long)b * 2 * hw + hw + pofs], px, py, Hs, Ws, tx, ty);
             if (regular) {
                 X0u = tx[0].fl;
                 Y0u = ty[0].fl;
-                build_window<K>(p, tx, ty, Hs, Ws, inv_kk, w, X0, Y0);
+                build_window<T, K>(p, tx, ty, Hs, Ws, inv_kk, w, X0, Y0);
             } else {
                 irr[atomicAdd(&nirr, 1)] = tid;
             }
         }
-        const __nv_bfloat16* s_b = src + (long long)b * Hs * Ws * C;
+        const T* s_b = src + (long long)b * Hs * Ws * C;
         // ldmatrix lane addresses
         const uint32_t g_frag_a = g_base + (warp * 32 + (lane & 15)) * GSTR + (lane >> 4) * 16;        // A = G rows
         const uint32_t s_frag_b = s_base + ((lane & 7) + ((lane >> 4) << 3)) * GSTR + ((lane >> 3) & 1) * 16;   // B = S rows
 
         for (int c0 = 0; c0 < C; c0 += CN) {
             if (c0 != 0) bar_sync(BT_BAR_PASS, BT_THREADS);       // the previous pass is done with G and the segments
-            load_g_tile<CN>(g_base, go_b, c0, C, gx0, gy0, H, W, tid);
+            load_g_tile<T, CN>(g_base, go_b, c0, C, gx0, gy0, H, W, tid);
             {
                 const int i = tid >> 3;
                 for (int j = tid & 7; j < CN / 8; j += 8)
@@ -270,7 +274,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                 if (yn <= by1) {
                     const int i = tid >> 3;
                     const uint32_t dst = s_base + (buf ^ 1) * (SEG * GSTR) + i * GSTR;
-                    const __nv_bfloat16* sp = s_b + ((long long)yn * Ws + min(xn + i, Ws - 1)) * C + c0;
+                    const T* sp = s_b + ((long long)yn * Ws + min(xn + i, Ws - 1)) * C + c0;
                     for (int j = tid & 7; j < CN / 8; j += 8) cp_async16(dst + j * 16, sp + j * 8);
                     cp_async_commit();
                 }
@@ -284,9 +288,9 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
 #pragma unroll
                             for (int q = 0; q < 4; ++q) pacc[mt][nt][q] = 0.f;
                     const uint32_t sf = s_frag_b + buf * (SEG * GSTR);
-                    if (pm == 3u) p_gemm<CN, true, true>(g_frag_a, sf, pacc);
-                    else if (pm == 1u) p_gemm<CN, true, false>(g_frag_a, sf, pacc);
-                    else p_gemm<CN, false, true>(g_frag_a, sf, pacc);
+                    if (pm == 3u) p_gemm<T, CN, true, true>(g_frag_a, sf, pacc);
+                    else if (pm == 1u) p_gemm<T, CN, true, false>(g_frag_a, sf, pacc);
+                    else p_gemm<T, CN, false, true>(g_frag_a, sf, pacc);
 #pragma unroll
                     for (int mt = 0; mt < 2; ++mt) {
                         if (((pm >> mt) & 1u) == 0u) continue;      // nobody reads the P rows of inactive pixels
@@ -325,7 +329,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
         // ---- regular pixels: grad_logits and grad_flow from Q (local_attn_pixel.cuh)
         if (regular) {
             float p[KK], dp[KK];
-            pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
+            pixel_softmax<T, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
             AxisTap<float> tx[K], ty[K];
             taps_regular<float, K>(flow[(long long)b * 2 * hw + pofs], flow[(long long)b * 2 * hw + hw + pofs], px, py, Hs, Ws, tx, ty);
             float gfx = 0.f, gfy = 0.f;
@@ -335,15 +339,15 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                 for (int j = 0; j < K; ++j)
                     dp[i * K + j] = tap_backward<float>(tx[j], ty[i], p[i * K + j] * inv_kk, inv_kk, Q[i * K1 + j], Q[i * K1 + j + 1],
                                                         Q[(i + 1) * K1 + j], Q[(i + 1) * K1 + j + 1], gfx, gfy);
-            store_pixel_grads<__nv_bfloat16, float, float, KK>(p, dp, KK, gfx, gfy, glogits + (long long)b * KK * hw + pofs,
-                                                               gflow + (long long)b * 2 * hw + pofs, hw, accumulate);
+            store_pixel_grads<T, float, float, KK>(p, dp, KK, gfx, gfy, glogits + (long long)b * KK * hw + pofs,
+                                                   gflow + (long long)b * 2 * hw + pofs, hw, accumulate);
         }
         // ---- pixels with non-consecutive taps: literal arithmetic, one pixel warp per pixel.  The grad_source warps
         // do not take part: within their register budget this path would spill, and such pixels are rare.
         const double2 fsc = DET ? fx_scale(fx_exp[b]) : make_double2(0.0, 0.0);
         for (int i = warp; i < nirr; i += 4) {
             const int m = irr[i];
-            irregular_pixel_bwd<K, DET>(src, flow, logits, gout, gsrc, gflow, glogits, b, C, Hs, Ws, H, W, gx0 + (m & 15),
+            irregular_pixel_bwd<T, K, DET>(src, flow, logits, gout, gsrc, gflow, glogits, b, C, Hs, Ws, H, W, gx0 + (m & 15),
                                         gy0 + (m >> 4), accumulate, lane, gsum, fsc);
         }
     } else {
@@ -354,11 +358,11 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
         group_decode(gcols, grows, b, gx0, gy0);
         group_bbox<K>(flow, b, gx0, gy0, H, W, Hs, Ws, lane, bx0, by0, bx1, by1);
         const long long hw = (long long)H * W;
-        const __nv_bfloat16* go_b = gout + (long long)b * hw * C;
+        const T* go_b = gout + (long long)b * hw * C;
         const int v = warp - 4, t = tid - 128;
         const uint32_t aw_frag = aw_base + (lane & 15) * BT_AWSTR + (lane >> 4) * 16;                  // A = Wfull^T
         const uint32_t g_frag_b = g_base + (lane & 15) * GSTR + (v * (CN / 4) + (lane >> 4) * 8) * 2;  // B = G (transposed)
-        __nv_bfloat16* gs_b = gsrc + (long long)b * Hs * Ws * C;
+        T* gs_b = gsrc + (long long)b * Hs * Ws * C;
         fx_t* gx_b = nullptr;
         double2 fsc = make_double2(0.0, 0.0);
         if constexpr (DET) {
@@ -368,7 +372,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
 
         for (int c0 = 0; c0 < C; c0 += CN) {
             if (c0 != 0) bar_sync(BT_BAR_PASS, BT_THREADS);       // the previous pass is done with G
-            load_g_tile<CN>(g_base, go_b, c0, C, gx0, gy0, H, W, tid);
+            load_g_tile<T, CN>(g_base, go_b, c0, C, gx0, gy0, H, W, tid);
             cp_async_wait_all();
             bar_sync(BT_BAR_PASS, BT_THREADS);                    // G complete
             for (int a = 0, y = by0, x = bx0; y <= by1;) {
@@ -396,8 +400,8 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                         for (int np = 0; np < NTW / 2; ++np) {
                             uint32_t bg[4];
                             ldsm_x4_t(g_frag_b + kk * 16 * GSTR + np * 32, bg);
-                            mma_bf16(gacc[2 * np], af, bg[0], bg[1]);
-                            mma_bf16(gacc[2 * np + 1], af, bg[2], bg[3]);
+                            mma16<T>(gacc[2 * np], af, bg[0], bg[1]);
+                            mma16<T>(gacc[2 * np + 1], af, bg[2], bg[3]);
                         }
                     }
                     bar_sync(BT_BAR_GS, 128);                     // every grad_source warp has read slab a
@@ -439,10 +443,10 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                         }
                     } else {
                         // grad_source of the segment.  Positions past the footprint add nothing and border positions add fp32
-                        // pairs to the scratch.  The others are rounded to bf16 pairs, regrouped within each quad so that a
+                        // pairs to the scratch.  The others are rounded to T pairs, regrouped within each quad so that a
                         // lane holds 8 consecutive channels of one position, and added 16 bytes at a time: per warp
                         // instruction, 8 positions x 64 contiguous bytes, two full 32-byte sectors each.
-                        uint32_t gv[2 * NTW];       // [h NTW + nt]: channels nt 8 + 2 tig, +1 of position x + gid + 8 h, as bf16 pair
+                        uint32_t gv[2 * NTW];       // [h NTW + nt]: channels nt 8 + 2 tig, +1 of position x + gid + 8 h, as T pair
 #pragma unroll
                         for (int h = 0; h < 2; ++h) {
                             const int xp = x + gid + 8 * h;
@@ -457,7 +461,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                             }
 #pragma unroll
                             for (int nt = 0; nt < NTW; ++nt) {
-                                const __nv_bfloat162 hv = __floats2bfloat162_rn(gacc[nt][2 * h], gacc[nt][2 * h + 1]);
+                                const typename Pair16<T>::type hv = floats2_rn<T>(gacc[nt][2 * h], gacc[nt][2 * h + 1]);
                                 gv[h * NTW + nt] = slot == -1 ? *reinterpret_cast<const uint32_t*>(&hv) : 0u;
                             }
                         }
@@ -467,7 +471,7 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                             quad_transpose(u, tig);
                             if ((u[0] | u[1] | u[2] | u[3]) != 0u) {        // all 8 values zero (or no position): nothing to add
                                 const int n = 4 * j + tig, h = n / NTW, nt = n % NTW;
-                                red_add_bf16x8(gs_b + ((long long)y * Ws + x + gid + 8 * h) * C + c0 + v * (CN / 4) + nt * 8, u);
+                                red_add_16x8(gs_b + ((long long)y * Ws + x + gid + 8 * h) * C + c0 + v * (CN / 4) + nt * 8, u);
                             }
                         }
                     }
@@ -482,8 +486,9 @@ k_local_attn_bwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
 
 // grad_source of the border positions: what the buffer holds (the caller's values, plus the irregular pixels' adds) plus
 // the fp32 sum of the groups' adds, rounded once.  One thread per (image, border slot, channel pair).
+template <typename T>
 __global__ void __launch_bounds__(256)
-k_fold_border(__nv_bfloat16* __restrict__ gsrc, const float* __restrict__ gborder, int B, int C, int Hs, int Ws) {
+k_fold_border(T* __restrict__ gsrc, const float* __restrict__ gborder, int B, int C, int Hs, int Ws) {
     const int nb = 2 * (Hs + Ws), c2 = C / 2;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long long)B * nb * c2) return;
@@ -496,28 +501,27 @@ k_fold_border(__nv_bfloat16* __restrict__ gsrc, const float* __restrict__ gborde
     else { y = s - 2 * Ws - Hs; x = Ws - 1; }
     if (border_slot(y, x, Hs, Ws) != s) return;       // a slot no position maps to (a corner, or Hs or Ws of 1)
     const float2 v = *reinterpret_cast<const float2*>(gborder + bs * C + c);
-    __nv_bfloat162* d = reinterpret_cast<__nv_bfloat162*>(gsrc + (((long long)b * Hs + y) * Ws + x) * C + c);
-    const float2 o = __bfloat1622float2(*d);
-    *d = __floats2bfloat162_rn(o.x + v.x, o.y + v.y);
+    typename Pair16<T>::type* d = reinterpret_cast<typename Pair16<T>::type*>(gsrc + (((long long)b * Hs + y) * Ws + x) * C + c);
+    const float2 o = pair_to_float2(*d);
+    *d = floats2_rn<T>(o.x + v.x, o.y + v.y);
 }
 
-template <int K, int CN, bool DET = false>
+template <int K, int CN, bool DET, typename T>
 static int launch_bwd(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow, void* glogits,
                       float* gborder, int B, int C, int Hs, int Ws, int H, int W, int accumulate, cudaStream_t st_,
                       fx_t* gsum = nullptr, const int* fx_exp = nullptr) {
     const int gcols = (W + GW - 1) / GW, grows = (H + GH - 1) / GH;
     const long long ngroups = (long long)B * gcols * grows;
     if (ngroups > INT_MAX) return GFLA_E_SHAPE;
-    auto kern = k_local_attn_bwd_tc<K, CN, DET>;
+    auto kern = k_local_attn_bwd_tc<K, CN, DET, T>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem<CN>::ALLOC);
     if (e != cudaSuccess) return static_cast<int>(e);
     kern<<<(unsigned)ngroups, BT_THREADS, BwdSmem<CN>::ALLOC, st_>>>(
-        (const __nv_bfloat16*)src, (const float*)flow, (const __nv_bfloat16*)logits, (const __nv_bfloat16*)gout, (__nv_bfloat16*)gsrc,
-        (float*)gflow, (__nv_bfloat16*)glogits, gborder, C, Hs, Ws, H, W, gcols, grows, accumulate, gsum, fx_exp);
+        (const T*)src, (const float*)flow, (const T*)logits, (const T*)gout, (T*)gsrc, (float*)gflow, (T*)glogits, gborder, C, Hs, Ws, H, W, gcols, grows, accumulate, gsum, fx_exp);
     const int st = launch_status();
     if (st != GFLA_OK || DET) return st;
     const long long n = (long long)B * 2 * (Hs + Ws) * (C / 2);
-    k_fold_border<<<(unsigned)((n + 255) / 256), 256, 0, st_>>>((__nv_bfloat16*)gsrc, gborder, B, C, Hs, Ws);
+    k_fold_border<T><<<(unsigned)((n + 255) / 256), 256, 0, st_>>>((T*)gsrc, gborder, B, C, Hs, Ws);
     return launch_status();
 }
 
@@ -557,14 +561,14 @@ static int pick_cn_bwd(int C) {
 
 bool local_attn_bwd_tc_supported(int C, int k, int dtype, int flow_dtype, int layout, const void* src, const void* gout,
                                  const void* gsrc) {
-    return dtype == GFLA_BF16 && flow_dtype == GFLA_F32 && layout == GFLA_NHWC && (k == 3 || k == 5) && pick_cn_bwd(C) != 0 &&
+    return (dtype == GFLA_BF16 || dtype == GFLA_F16) && flow_dtype == GFLA_F32 && layout == GFLA_NHWC && (k == 3 || k == 5) && pick_cn_bwd(C) != 0 &&
            aligned(src, 16) && aligned(gout, 16) && aligned(gsrc, 16);
 }
 
 // accumulate = 0: grad_source is zero-filled here and all three gradients are overwritten; 1: everything is added into the
 // caller's buffers
 int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow, void* glogits,
-                      int B, int C, int Hs, int Ws, int H, int W, int k, int accumulate, cudaStream_t st_) {
+                      int B, int C, int Hs, int Ws, int H, int W, int k, int dtype, int accumulate, cudaStream_t st_) {
     if (!accumulate) {
         const int z = zero_async(gsrc, (size_t)B * C * Hs * Ws * 2, st_);
         if (z != GFLA_OK) return z;
@@ -578,10 +582,15 @@ int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, con
     if (e != cudaSuccess) return static_cast<int>(e);
     int r = zero_async(gborder, border_bytes, st_);
     if (r == GFLA_OK) {
-#define GFLA_BT_CASE(K_, CN_) \
-        if (k == K_ && cn == CN_) r = tc::launch_bwd<K_, CN_>(src, flow, logits, gout, gsrc, gflow, glogits, gborder, B, C, Hs, Ws, H, W, accumulate, st_);
-        GFLA_BT_CASE(5, 256) GFLA_BT_CASE(5, 128) GFLA_BT_CASE(5, 64)
-        GFLA_BT_CASE(3, 256) GFLA_BT_CASE(3, 128) GFLA_BT_CASE(3, 64)
+#define GFLA_BT_CASE(T_, K_, CN_) \
+        if (k == K_ && cn == CN_) r = tc::launch_bwd<K_, CN_, false, T_>(src, flow, logits, gout, gsrc, gflow, glogits, gborder, B, C, Hs, Ws, H, W, accumulate, st_);
+        if (dtype == GFLA_F16) {
+            GFLA_BT_CASE(__half, 5, 256) GFLA_BT_CASE(__half, 5, 128) GFLA_BT_CASE(__half, 5, 64)
+            GFLA_BT_CASE(__half, 3, 256) GFLA_BT_CASE(__half, 3, 128) GFLA_BT_CASE(__half, 3, 64)
+        } else {
+            GFLA_BT_CASE(__nv_bfloat16, 5, 256) GFLA_BT_CASE(__nv_bfloat16, 5, 128) GFLA_BT_CASE(__nv_bfloat16, 5, 64)
+            GFLA_BT_CASE(__nv_bfloat16, 3, 256) GFLA_BT_CASE(__nv_bfloat16, 3, 128) GFLA_BT_CASE(__nv_bfloat16, 3, 64)
+        }
 #undef GFLA_BT_CASE
     }
     e = cudaFreeAsync(gborder, st_);
@@ -591,13 +600,19 @@ int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, con
 // grad_source into the fixed-point sums gsum (zeroed, channels-last, exponents in fx_exp: det_accum.cuh); no border scratch
 // and no k_fold_border.  grad_flow / grad_logits follow `accumulate` as above.
 int local_attn_bwd_tc_det(const void* src, const void* flow, const void* logits, const void* gout, void* gflow, void* glogits, int B,
-                          int C, int Hs, int Ws, int H, int W, int k, int accumulate, fx_t* gsum, const int* fx_exp, cudaStream_t st_) {
+                          int C, int Hs, int Ws, int H, int W, int k, int dtype, int accumulate, fx_t* gsum, const int* fx_exp,
+                          cudaStream_t st_) {
     const int cn = pick_cn_bwd(C);
-#define GFLA_BT_CASE(K_, CN_) \
-    if (k == K_ && cn == CN_) return tc::launch_bwd<K_, CN_, true>(src, flow, logits, gout, nullptr, gflow, glogits, nullptr, B, C, Hs, Ws, \
-                                                                   H, W, accumulate, st_, gsum, fx_exp);
-    GFLA_BT_CASE(5, 256) GFLA_BT_CASE(5, 128) GFLA_BT_CASE(5, 64)
-    GFLA_BT_CASE(3, 256) GFLA_BT_CASE(3, 128) GFLA_BT_CASE(3, 64)
+#define GFLA_BT_CASE(T_, K_, CN_) \
+    if (k == K_ && cn == CN_) return tc::launch_bwd<K_, CN_, true, T_>(src, flow, logits, gout, nullptr, gflow, glogits, nullptr, B, C, Hs, \
+                                                                       Ws, H, W, accumulate, st_, gsum, fx_exp);
+    if (dtype == GFLA_F16) {
+        GFLA_BT_CASE(__half, 5, 256) GFLA_BT_CASE(__half, 5, 128) GFLA_BT_CASE(__half, 5, 64)
+        GFLA_BT_CASE(__half, 3, 256) GFLA_BT_CASE(__half, 3, 128) GFLA_BT_CASE(__half, 3, 64)
+    } else {
+        GFLA_BT_CASE(__nv_bfloat16, 5, 256) GFLA_BT_CASE(__nv_bfloat16, 5, 128) GFLA_BT_CASE(__nv_bfloat16, 5, 64)
+        GFLA_BT_CASE(__nv_bfloat16, 3, 256) GFLA_BT_CASE(__nv_bfloat16, 3, 128) GFLA_BT_CASE(__nv_bfloat16, 3, 64)
+    }
 #undef GFLA_BT_CASE
     return GFLA_E_NOTSUP;
 }

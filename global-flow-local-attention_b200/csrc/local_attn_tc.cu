@@ -1,4 +1,5 @@
-// Fused local-attention forward on the tensor cores (bf16 data, fp32 flow, k in {3, 5}, NCHW or channels-last).
+// Fused local-attention forward on the tensor cores (bf16 or fp16 data, fp32 flow, k in {3, 5}, NCHW or channels-last).
+// T, the data's 16-bit type, is also the type of the weight slab, so both MMA operands are T; the accumulators are fp32.
 //
 // Per 16x8 pixel group the weighted gather is a dense GEMM
 //     out[128 px][C] = Wfull[128 px][footprint] * S[footprint][C]
@@ -6,7 +7,7 @@
 // K-steps for channels-last, 16 for planar):
 //   * one thread per pixel: softmax, taps (exactly like block_extractor_kernel.cu:62-76), the collapsed (k+1)^2 window
 //     (tile_window.cuh) kept in registers;
-//   * per step every pixel thread writes its pixel's row of the weight slab A[128 px][NPOS] (bf16; at most k+1 non-zeros);
+//   * per step every pixel thread writes its pixel's row of the weight slab A[128 px][NPOS] (T; at most k+1 non-zeros);
 //     the source segment B[NPOS][CN ch] is staged ahead;
 //   * the warp that owns pixel rows 32w..32w+31 multiplies them with mma.sync m16n8k16 (fp32 accumulators in registers),
 //     skipping per K-step the 16-pixel m-tiles none of whose windows meets it (window_meets_step: their slab rows are all
@@ -25,7 +26,7 @@ namespace tc {
 constexpr int FT_THREADS = 128;                 // one thread per pixel of the group
 constexpr int FT_CN = 64;                       // channels per pass (N of the MMAs)
 constexpr int FT_BSTR = FT_CN * 2 + 16;         // source-segment row: 128 B + 16 B pad
-constexpr int FT_ASTR = SEG * 2 + 16;           // weight-slab row: SEG bf16 + 16 B pad (conflict-free ldmatrix)
+constexpr int FT_ASTR = SEG * 2 + 16;           // weight-slab row: SEG 16-bit weights + 16 B pad (conflict-free ldmatrix)
 constexpr int FT_BSEG = SEG * FT_BSTR;          // one source segment in shared memory
 
 struct FwdSmem {
@@ -37,11 +38,13 @@ struct FwdSmem {
 
 // source row segment (16 positions from x, clamped at the right edge: those columns carry zero weight) x 64 channels,
 // loaded into registers one step ahead and stored to shared memory after the step's MMAs
+template <typename T>
 struct SegRegs {
-    __nv_bfloat16 v[8];
+    T v[8];
 };
-__device__ __forceinline__ void seg_load(const __nv_bfloat16* __restrict__ src, int b, int C, int c0, int Hs, int Ws, int y, int x,
-                                         int tid, SegRegs& r) {
+template <typename T>
+__device__ __forceinline__ void seg_load(const T* __restrict__ src, int b, int C, int c0, int Hs, int Ws, int y, int x, int tid,
+                                         SegRegs<T>& r) {
 #pragma unroll
     for (int it = 0; it < 8; ++it) {
         const int idx = it * FT_THREADS + tid, c = idx >> 4, i = idx & 15;
@@ -49,7 +52,8 @@ __device__ __forceinline__ void seg_load(const __nv_bfloat16* __restrict__ src, 
         r.v[it] = src[(((long long)b * C + c0 + c) * Hs + y) * Ws + xs];
     }
 }
-__device__ __forceinline__ void seg_store(uint32_t dst, int tid, const SegRegs& r) {
+template <typename T>
+__device__ __forceinline__ void seg_store(uint32_t dst, int tid, const SegRegs<T>& r) {
 #pragma unroll
     for (int it = 0; it < 8; ++it) {
         const int idx = it * FT_THREADS + tid, c = idx >> 4, i = idx & 15;
@@ -57,11 +61,11 @@ __device__ __forceinline__ void seg_store(uint32_t dst, int tid, const SegRegs& 
     }
 }
 
-template <int K>
+template <int K, typename T>
 __global__ void __launch_bounds__(FT_THREADS, 1)
-k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow, const __nv_bfloat16* __restrict__ logits,
-                    __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ probs, const __nv_bfloat16* __restrict__ prev,
-                    const __nv_bfloat16* __restrict__ mask, int C, int Hs, int Ws, int H, int W, int gcols, int grows) {
+k_local_attn_fwd_tc(const T* __restrict__ src, const float* __restrict__ flow, const T* __restrict__ logits, T* __restrict__ out,
+                    T* __restrict__ probs, const T* __restrict__ prev, const T* __restrict__ mask, int C, int Hs, int Ws, int H, int W,
+                    int gcols, int grows) {
     constexpr int K1 = K + 1, KK = K * K;
     __shared__ FwdSmem sm;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, gid = lane >> 2, tig = lane & 3;
@@ -84,14 +88,14 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     if (valid) {
         const long long pofs = (long long)py * W + px;
         float p[KK];
-        pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
+        pixel_softmax<T, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
         if (probs != nullptr) {
 #pragma unroll
-            for (int t = 0; t < KK; ++t) probs[(long long)b * KK * hw + t * hw + pofs] = __float2bfloat16_rn(p[t]);
+            for (int t = 0; t < KK; ++t) st(probs + (long long)b * KK * hw + t * hw + pofs, p[t]);
         }
         AxisTap<float> tx[K], ty[K];
         regular = taps_regular<float, K>(flow[(long long)b * 2 * hw + pofs], flow[(long long)b * 2 * hw + hw + pofs], px, py, Hs, Ws, tx, ty);
-        if (regular) build_window<K>(p, tx, ty, Hs, Ws, 1.0f / static_cast<float>(KK), w, X0, Y0);
+        if (regular) build_window<T, K>(p, tx, ty, Hs, Ws, 1.0f / static_cast<float>(KK), w, X0, Y0);
         else sm.irr[atomicAdd(&sm.nirr, 1)] = tid;
     }
 
@@ -108,7 +112,7 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
             for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
                 for (int q = 0; q < 4; ++q) acc[mt][nt][q] = 0.f;
-        SegRegs pend;
+        SegRegs<T> pend;
         __syncthreads();      // the previous pass's MMAs are done with both buffers
         seg_load(src, b, C, c0, Hs, Ws, by0, bx0, tid, pend);
         seg_store(b_base, tid, pend);
@@ -141,8 +145,8 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
 #pragma unroll
                     for (int mt = 0; mt < 2; ++mt) {
                         if (((wm >> mt) & 1u) == 0u) continue;
-                        mma_bf16(acc[mt][2 * np], af[mt], bf[0], bf[1]);
-                        mma_bf16(acc[mt][2 * np + 1], af[mt], bf[2], bf[3]);
+                        mma16<T>(acc[mt][2 * np], af[mt], bf[0], bf[1]);
+                        mma16<T>(acc[mt][2 * np + 1], af[mt], bf[2], bf[3]);
                     }
                 }
             }
@@ -162,18 +166,18 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
                 bool irr = false;
                 for (int i = 0; i < sm.nirr; ++i) irr |= sm.irr[i] == m;
                 if (irr) continue;
-                const float qm = prev != nullptr ? __bfloat162float(mask[(long long)b * hw + qofs]) : 1.f;
+                const float qm = prev != nullptr ? ld(mask + (long long)b * hw + qofs) : 1.f;
 #pragma unroll
                 for (int nt = 0; nt < 8; ++nt) {
                     const int c = c0 + nt * 8 + 2 * tig;
                     float v0 = acc[mt][nt][2 * h], v1 = acc[mt][nt][2 * h + 1];
                     const long long o0 = ((long long)b * C + c) * hw + qofs, o1 = o0 + hw;
                     if (prev != nullptr) {
-                        v0 = __bfloat162float(prev[o0]) * (1.f - qm) + v0 * qm;
-                        v1 = __bfloat162float(prev[o1]) * (1.f - qm) + v1 * qm;
+                        v0 = ld(prev + o0) * (1.f - qm) + v0 * qm;
+                        v1 = ld(prev + o1) * (1.f - qm) + v1 * qm;
                     }
-                    out[o0] = __float2bfloat16_rn(v0);
-                    out[o1] = __float2bfloat16_rn(v1);
+                    st(out + o0, v0);
+                    st(out + o1, v1);
                 }
             }
     }
@@ -181,7 +185,7 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
     for (int i = warp; i < sm.nirr; i += FT_THREADS / 32) {
         const int m = sm.irr[i], qx = gx0 + (m & 15), qy = gy0 + (m >> 4);
         const long long qofs = (long long)qy * W + qx;
-        irregular_pixel<K, false>(src, logits, out, prev, mask, b, C, Hs, Ws, H, W, qx, qy, flow[(long long)b * 2 * hw + qofs],
+        irregular_pixel<T, K, false>(src, logits, out, prev, mask, b, C, Hs, Ws, H, W, qx, qy, flow[(long long)b * 2 * hw + qofs],
                                   flow[(long long)b * 2 * hw + hw + qofs], lane);
     }
 }
@@ -189,7 +193,7 @@ k_local_attn_fwd_tc(const __nv_bfloat16* __restrict__ src, const float* __restri
 // ------------------------------------------------------------------ channels-last
 constexpr int FC_THREADS = 256;                 // pixel warpgroup (warps 0-3) + MMA warpgroup (warps 4-7)
 constexpr int FC_NPOS = 2 * SEG;                // source positions per step: two MMA K-steps
-constexpr int FC_ASTR = FC_NPOS * 2 + 16;       // weight-slab row: 32 bf16 + 16 B pad (conflict-free ldmatrix)
+constexpr int FC_ASTR = FC_NPOS * 2 + 16;       // weight-slab row: 32 16-bit weights + 16 B pad (conflict-free ldmatrix)
 constexpr int FC_NA = 3;                        // weight slabs (and row-bit words) in rotation
 constexpr int FC_AHEAD = 3;                     // source segments in flight ahead of the step that writes its slab
 constexpr int FC_NSEG = FC_AHEAD + FC_NA;       // ring slots: step s's slot is refilled once FREE of step s shows it read
@@ -201,7 +205,7 @@ constexpr int FC_BAR_FREE = 4;                  // + slab: slab and segment read
 
 template <int CN>
 struct FwdClSmem {
-    static constexpr int BSTR = CN * 2 + 16;             // source-segment row: CN bf16 + 16 B pad
+    static constexpr int BSTR = CN * 2 + 16;             // source-segment row: CN 16-bit values + 16 B pad
     static constexpr int BSEG = FC_NPOS * BSTR;          // one ring slot
     static constexpr int A = 0;
     static constexpr int B = A + FC_NA * 128 * FC_ASTR;
@@ -214,13 +218,13 @@ struct FwdClSmem {
 // positions, clamped at the right edge like the planar segment) with cp.async and moves the cursor on in the steps'
 // order: row-major over the footprint, then on into the next CN-channel pass.  Past the last pass it copies nothing, but
 // it commits a group on every call, so that the wait count before each FULL holds to the end.
-template <int CN>
-__device__ __forceinline__ void seg_produce(const __nv_bfloat16* __restrict__ src, int b, int C, int Hs, int Ws, int bx0, int by0,
+template <typename T, int CN>
+__device__ __forceinline__ void seg_produce(const T* __restrict__ src, int b, int C, int Hs, int Ws, int bx0, int by0,
                                             int bx1, int by1, int& c0, int& y, int& x, uint32_t dst, int t) {
     constexpr int CH = CN / 8;                            // 16-byte chunks per position
     if (c0 < C) {
         const int j = t % CH;
-        const __nv_bfloat16* row = src + ((long long)b * Hs + y) * Ws * C + c0 + j * 8;
+        const T* row = src + ((long long)b * Hs + y) * Ws * C + c0 + j * 8;
 #pragma unroll
         for (int i = t / CH; i < FC_NPOS; i += 128 / CH)   // position
             cp_async16(dst + i * FwdClSmem<CN>::BSTR + j * 16, row + (long long)min(x + i, Ws - 1) * C);
@@ -241,11 +245,11 @@ __device__ __forceinline__ void seg_produce(const __nv_bfloat16* __restrict__ sr
 //     the slab rows pixel warp v wrote), signalled by FREE; the epilogue and the irregular pixels.
 // The pixel warpgroup waits for FREE of step s - 3 before it writes slab s, so it runs up to two steps ahead, also across
 // passes.  Steps are numbered across all passes; every slab is zero at the start of each step.
-template <int K, int CN>
+template <int K, int CN, typename T>
 __global__ void __launch_bounds__(FC_THREADS, 2)
-k_local_attn_fwd_tc_cl(const __nv_bfloat16* __restrict__ src, const float* __restrict__ flow, const __nv_bfloat16* __restrict__ logits,
-                       __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ probs, const __nv_bfloat16* __restrict__ prev,
-                       const __nv_bfloat16* __restrict__ mask, int C, int Hs, int Ws, int H, int W, int gcols, int grows) {
+k_local_attn_fwd_tc_cl(const T* __restrict__ src, const float* __restrict__ flow, const T* __restrict__ logits, T* __restrict__ out,
+                       T* __restrict__ probs, const T* __restrict__ prev, const T* __restrict__ mask, int C, int Hs, int Ws, int H,
+                       int W, int gcols, int grows) {
     constexpr int K1 = K + 1, KK = K * K;
     using L = FwdClSmem<CN>;
     extern __shared__ __align__(16) unsigned char smem[];
@@ -269,7 +273,7 @@ k_local_attn_fwd_tc_cl(const __nv_bfloat16* __restrict__ src, const float* __res
         int nc0 = 0, ny = by0, nx = bx0;   // the ring's cursor: FC_AHEAD segments ahead of the steps
 #pragma unroll
         for (int i = 0; i < FC_AHEAD; ++i)
-            seg_produce<CN>(src, b, C, Hs, Ws, bx0, by0, bx1, by1, nc0, ny, nx, b_base + i * L::BSEG, tid);
+            seg_produce<T, CN>(src, b, C, Hs, Ws, bx0, by0, bx1, by1, nc0, ny, nx, b_base + i * L::BSEG, tid);
         const long long hw = (long long)H * W;
         const int px = gx0 + (tid & 15), py = gy0 + (tid >> 4);
         uint32_t w[K1 * K1 / 2];
@@ -278,14 +282,14 @@ k_local_attn_fwd_tc_cl(const __nv_bfloat16* __restrict__ src, const float* __res
         if (px < W && py < H) {
             const long long pofs = (long long)py * W + px;
             float p[KK];
-            pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
+            pixel_softmax<T, float, KK>(logits + (long long)b * KK * hw + pofs, hw, KK, p);
             if (probs != nullptr) {
 #pragma unroll
-                for (int t = 0; t < KK; ++t) probs[(long long)b * KK * hw + t * hw + pofs] = __float2bfloat16_rn(p[t]);
+                for (int t = 0; t < KK; ++t) st(probs + (long long)b * KK * hw + t * hw + pofs, p[t]);
             }
             AxisTap<float> tx[K], ty[K];
             regular = taps_regular<float, K>(flow[(long long)b * 2 * hw + pofs], flow[(long long)b * 2 * hw + hw + pofs], px, py, Hs, Ws, tx, ty);
-            if (regular) build_window<K>(p, tx, ty, Hs, Ws, 1.0f / static_cast<float>(KK), w, X0, Y0);
+            if (regular) build_window<T, K>(p, tx, ty, Hs, Ws, 1.0f / static_cast<float>(KK), w, X0, Y0);
             else irr[atomicAdd(&nirr, 1)] = tid;
         }
         // the window is built: the steady state needs only the window, its origin and the walk
@@ -297,7 +301,7 @@ k_local_attn_fwd_tc_cl(const __nv_bfloat16* __restrict__ src, const float* __res
                 // slab a and the segment of step s - 3 are read, the slab is zeroed
                 if (s >= FC_NA) bar_sync(FC_BAR_FREE + a, FC_THREADS);
                 // so step s - 3's slot, (s + FC_AHEAD) % FC_NSEG, takes the segment of step s + FC_AHEAD
-                seg_produce<CN>(src, b, C, Hs, Ws, bx0, by0, bx1, by1, nc0, ny, nx, b_base + slot * L::BSEG, tid);
+                seg_produce<T, CN>(src, b, C, Hs, Ws, bx0, by0, bx1, by1, nc0, ny, nx, b_base + slot * L::BSEG, tid);
                 slot = slot == FC_NSEG - 1 ? 0 : slot + 1;
                 // per MMA K-step (SEG positions): the m-tiles of this warp with an active pixel
                 uint32_t bits = 0u;
@@ -370,8 +374,8 @@ k_local_attn_fwd_tc_cl(const __nv_bfloat16* __restrict__ src, const float* __res
 #pragma unroll
                             for (int mt = 0; mt < 2; ++mt) {
                                 if (((wm >> mt) & 1u) == 0u) continue;
-                                mma_bf16(acc[mt][2 * np], af[mt], bf[np & 1][0], bf[np & 1][1]);
-                                mma_bf16(acc[mt][2 * np + 1], af[mt], bf[np & 1][2], bf[np & 1][3]);
+                                mma16<T>(acc[mt][2 * np], af[mt], bf[np & 1][0], bf[np & 1][1]);
+                                mma16<T>(acc[mt][2 * np + 1], af[mt], bf[np & 1][2], bf[np & 1][3]);
                             }
                         }
                     }
@@ -401,17 +405,17 @@ k_local_attn_fwd_tc_cl(const __nv_bfloat16* __restrict__ src, const float* __res
                     bool ir = false;
                     for (int i = 0; i < nirr; ++i) ir |= irr[i] == m;
                     if (ir) continue;
-                    const float qm = prev != nullptr ? __bfloat162float(mask[(long long)b * hw + qofs]) : 1.f;
+                    const float qm = prev != nullptr ? ld(mask + (long long)b * hw + qofs) : 1.f;
 #pragma unroll
                     for (int nt = 0; nt < CN / 8; ++nt) {
                         const int c = c0 + nt * 8 + 2 * tig;
                         float v0 = acc[mt][nt][2 * h], v1 = acc[mt][nt][2 * h + 1];
                         const long long o0 = ((long long)b * hw + qofs) * C + c;
                         if (prev != nullptr) {
-                            v0 = __bfloat162float(prev[o0]) * (1.f - qm) + v0 * qm;
-                            v1 = __bfloat162float(prev[o0 + 1]) * (1.f - qm) + v1 * qm;
+                            v0 = ld(prev + o0) * (1.f - qm) + v0 * qm;
+                            v1 = ld(prev + o0 + 1) * (1.f - qm) + v1 * qm;
                         }
-                        *reinterpret_cast<__nv_bfloat162*>(out + o0) = __floats2bfloat162_rn(v0, v1);
+                        *reinterpret_cast<typename Pair16<T>::type*>(out + o0) = floats2_rn<T>(v0, v1);
                     }
                 }
         }
@@ -420,36 +424,36 @@ k_local_attn_fwd_tc_cl(const __nv_bfloat16* __restrict__ src, const float* __res
         for (int i = v; i < nirr; i += 4) {
             const int m = irr[i], qx = gx0 + (m & 15), qy = gy0 + (m >> 4);
             const long long qofs = (long long)qy * W + qx;
-            irregular_pixel<K, true>(src, logits, out, prev, mask, b, C, Hs, Ws, H, W, qx, qy, flow[(long long)b * 2 * hw + qofs],
+            irregular_pixel<T, K, true>(src, logits, out, prev, mask, b, C, Hs, Ws, H, W, qx, qy, flow[(long long)b * 2 * hw + qofs],
                                      flow[(long long)b * 2 * hw + hw + qofs], lane);
         }
     }
 }
 
-template <int K>
+template <int K, typename T>
 static int launch_fwd(const void* src, const void* flow, const void* logits, void* out, void* probs, const void* prev, const void* mask,
                       int B, int C, int Hs, int Ws, int H, int W, cudaStream_t st_) {
     const int gcols = (W + GW - 1) / GW, grows = (H + GH - 1) / GH;
     const long long ngroups = (long long)B * gcols * grows;
     if (ngroups > INT_MAX) return GFLA_E_SHAPE;
-    k_local_attn_fwd_tc<K><<<(unsigned)ngroups, FT_THREADS, 0, st_>>>(
-        (const __nv_bfloat16*)src, (const float*)flow, (const __nv_bfloat16*)logits, (__nv_bfloat16*)out, (__nv_bfloat16*)probs,
-        (const __nv_bfloat16*)prev, (const __nv_bfloat16*)mask, C, Hs, Ws, H, W, gcols, grows);
+    k_local_attn_fwd_tc<K, T><<<(unsigned)ngroups, FT_THREADS, 0, st_>>>((const T*)src, (const float*)flow, (const T*)logits, (T*)out,
+                                                                        (T*)probs, (const T*)prev, (const T*)mask, C, Hs, Ws, H, W,
+                                                                        gcols, grows);
     return launch_status();
 }
 
-template <int K, int CN>
+template <int K, int CN, typename T>
 static int launch_fwd_cl(const void* src, const void* flow, const void* logits, void* out, void* probs, const void* prev,
                          const void* mask, int B, int C, int Hs, int Ws, int H, int W, cudaStream_t st_) {
     const int gcols = (W + GW - 1) / GW, grows = (H + GH - 1) / GH;
     const long long ngroups = (long long)B * gcols * grows;
     if (ngroups > INT_MAX) return GFLA_E_SHAPE;
-    auto kern = k_local_attn_fwd_tc_cl<K, CN>;
+    auto kern = k_local_attn_fwd_tc_cl<K, CN, T>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdClSmem<CN>::ALLOC);
     if (e != cudaSuccess) return static_cast<int>(e);
-    kern<<<(unsigned)ngroups, FC_THREADS, FwdClSmem<CN>::ALLOC, st_>>>(
-        (const __nv_bfloat16*)src, (const float*)flow, (const __nv_bfloat16*)logits, (__nv_bfloat16*)out, (__nv_bfloat16*)probs,
-        (const __nv_bfloat16*)prev, (const __nv_bfloat16*)mask, C, Hs, Ws, H, W, gcols, grows);
+    kern<<<(unsigned)ngroups, FC_THREADS, FwdClSmem<CN>::ALLOC, st_>>>((const T*)src, (const float*)flow, (const T*)logits, (T*)out,
+                                                                       (T*)probs, (const T*)prev, (const T*)mask, C, Hs, Ws, H, W,
+                                                                       gcols, grows);
     return launch_status();
 }
 
@@ -457,24 +461,32 @@ static int launch_fwd_cl(const void* src, const void* flow, const void* logits, 
 
 bool local_attn_fwd_tc_supported(int C, int Ws, int k, int dtype, int flow_dtype, int layout, const void* src, const void* out) {
     const bool c_ok = C % 256 == 0 || C == 128 || C == 64;
-    if (!(dtype == GFLA_BF16 && flow_dtype == GFLA_F32 && (k == 3 || k == 5) && c_ok && aligned(src, 16))) return false;
+    if (!((dtype == GFLA_BF16 || dtype == GFLA_F16) && flow_dtype == GFLA_F32 && (k == 3 || k == 5) && c_ok && aligned(src, 16))) return false;
     // channels-last: 16-byte cp.async of the source and 4-byte channel-pair stores need aligned pointers
     return layout == GFLA_NHWC ? aligned(out, 16) : (Ws % 8) == 0;
+}
+
+template <typename T>
+static int local_attn_fwd_tc_t(const void* src, const void* flow, const void* logits, void* out, void* probs, const void* prev,
+                               const void* mask, int B, int C, int Hs, int Ws, int H, int W, int k, int layout, cudaStream_t st_) {
+    if (layout != GFLA_NHWC) return k == 5 ? tc::launch_fwd<5, T>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, st_)
+                                           : tc::launch_fwd<3, T>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, st_);
+    // channels-last: 128-channel passes wherever C allows them (C = 64 takes one 64-channel pass)
+    const bool wide = C % 128 == 0;
+#define GFLA_FC_CASE(K_, CN_) \
+    if (k == K_ && wide == (CN_ == 128)) return tc::launch_fwd_cl<K_, CN_, T>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, st_);
+    GFLA_FC_CASE(5, 128) GFLA_FC_CASE(5, 64) GFLA_FC_CASE(3, 128) GFLA_FC_CASE(3, 64)
+#undef GFLA_FC_CASE
+    return GFLA_E_NOTSUP;
 }
 
 int local_attn_fwd_tc(const void* src, const void* flow, const void* logits, void* out, void* probs, const void* prev,
                       const void* mask, int B, int C, int Hs, int Ws, int H, int W, int k, int dtype, int flow_dtype,
                       int layout, cudaStream_t st_) {
     if (!local_attn_fwd_tc_supported(C, Ws, k, dtype, flow_dtype, layout, src, out)) return GFLA_E_NOTSUP;
-    if (layout != GFLA_NHWC) return k == 5 ? tc::launch_fwd<5>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, st_)
-                                           : tc::launch_fwd<3>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, st_);
-    // channels-last: 128-channel passes wherever C allows them (C = 64 takes one 64-channel pass)
-    const bool wide = C % 128 == 0;
-#define GFLA_FC_CASE(K_, CN_) \
-    if (k == K_ && wide == (CN_ == 128)) return tc::launch_fwd_cl<K_, CN_>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, st_);
-    GFLA_FC_CASE(5, 128) GFLA_FC_CASE(5, 64) GFLA_FC_CASE(3, 128) GFLA_FC_CASE(3, 64)
-#undef GFLA_FC_CASE
-    return GFLA_E_NOTSUP;
+    return dtype == GFLA_F16 ? local_attn_fwd_tc_t<__half>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, k, layout, st_)
+                             : local_attn_fwd_tc_t<__nv_bfloat16>(src, flow, logits, out, probs, prev, mask, B, C, Hs, Ws, H, W, k, layout,
+                                                                  st_);
 }
 
 }  // namespace gfla

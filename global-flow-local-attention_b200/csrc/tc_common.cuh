@@ -1,7 +1,8 @@
 // sm_90a building blocks shared by the tensor-core tile kernels: cp.async staging, ldmatrix fragment loads and
-// the warp-level bf16 MMA (m16n8k16, fp32 accumulate).  Raw PTX, no CUTLASS dependency.
+// the warp-level bf16 and fp16 MMAs (m16n8k16, fp32 accumulate).  Raw PTX, no CUTLASS dependency.
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -71,6 +72,42 @@ __device__ __forceinline__ uint32_t bf16_bits(float v) {
     const __nv_bfloat16 h = __float2bfloat16_rn(v);
     return static_cast<uint32_t>(*reinterpret_cast<const unsigned short*>(&h));
 }
+
+// ------------------------------------------------------------------ the 16-bit element type T of the local-attention
+// tile kernels: __nv_bfloat16 or __half.  Both MMA operands are T; accumulation is fp32 either way.
+// D (+)= A[16x16, row] * B[16x8, col], fp16 in, fp32 accumulate (warp-collective)
+__device__ __forceinline__ void mma_f16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ uint32_t f16_bits(float v) {
+    const __half h = __float2half_rn(v);
+    return static_cast<uint32_t>(*reinterpret_cast<const unsigned short*>(&h));
+}
+
+template <typename T> struct Pair16;
+template <> struct Pair16<__nv_bfloat16> { using type = __nv_bfloat162; };
+template <> struct Pair16<__half> { using type = __half2; };
+
+template <typename T> __device__ __forceinline__ void mma16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1);
+template <> __device__ __forceinline__ void mma16<__nv_bfloat16>(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    mma_bf16(d, a, b0, b1);
+}
+template <> __device__ __forceinline__ void mma16<__half>(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    mma_f16(d, a, b0, b1);
+}
+// the bits of v rounded to T (round to nearest even; fp16 keeps subnormals), in the low half
+template <typename T> __device__ __forceinline__ uint32_t bits16(float v);
+template <> __device__ __forceinline__ uint32_t bits16<__nv_bfloat16>(float v) { return bf16_bits(v); }
+template <> __device__ __forceinline__ uint32_t bits16<__half>(float v) { return f16_bits(v); }
+// (a, b) rounded to a T pair, a in the low half
+template <typename T> __device__ __forceinline__ typename Pair16<T>::type floats2_rn(float a, float b);
+template <> __device__ __forceinline__ __nv_bfloat162 floats2_rn<__nv_bfloat16>(float a, float b) { return __floats2bfloat162_rn(a, b); }
+template <> __device__ __forceinline__ __half2 floats2_rn<__half>(float a, float b) { return __floats2half2_rn(a, b); }
+__device__ __forceinline__ float2 pair_to_float2(__nv_bfloat162 v) { return __bfloat1622float2(v); }
+__device__ __forceinline__ float2 pair_to_float2(__half2 v) { return __half22float2(v); }
 
 // Division of group indices by run-time image geometry: magic multiplier computed once, then umulhi + shift per use.
 // Exact for 0 <= n < 2^31, d >= 1.

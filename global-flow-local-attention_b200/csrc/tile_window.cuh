@@ -1,5 +1,6 @@
 // Pieces shared by the forward and backward tile kernels: pixel-group geometry, the collapsed (k+1)x(k+1) weight
-// window and its scatter into the bf16 weight slab, and the literal path of pixels whose taps are not consecutive.
+// window and its scatter into the 16-bit weight slab, and the literal path of pixels whose taps are not consecutive.
+// T, the 16-bit element type of the data and of the weight slab, is __nv_bfloat16 or __half.
 #pragma once
 #include <climits>
 
@@ -64,9 +65,9 @@ __device__ __forceinline__ void group_bbox(const float* __restrict__ flow, int b
 // p = softmax probabilities (already scaled by whatever the caller wants, e.g. 1/k^2).  Border handling =
 // the reference's index clamp: weights of out-of-range columns / rows are folded onto the border position.
 // On return X0 / Y0 are shifted so that the mapping also holds for windows lying entirely outside the image.
-// The kernels only ever store the weights as bf16, so the window comes back as bf16 pairs: wp[r (K+1)/2 + s/2]
-// holds w[r][s] in its low half for even s, in its high half for odd s.
-template <int K>
+// The kernels only ever store the weights as T, so the window comes back as T pairs: wp[r (K+1)/2 + s/2] holds w[r][s]
+// in its low half for even s, in its high half for odd s.
+template <typename T, int K>
 __device__ __forceinline__ void build_window(const float* p, const AxisTap<float> (&tx)[K], const AxisTap<float> (&ty)[K],
                                              int Hs, int Ws, float scale, uint32_t (&wp)[(K + 1) * (K + 1) / 2], int& X0, int& Y0) {
     constexpr int K1 = K + 1;
@@ -117,15 +118,15 @@ __device__ __forceinline__ void build_window(const float* p, const AxisTap<float
         Y0 = min(max(Y0, -K), Hs - 1);
     }
 #pragma unroll
-    for (int i = 0; i < K1 * K1 / 2; ++i) wp[i] = bf16_bits(w[2 * i]) | (bf16_bits(w[2 * i + 1]) << 16);
+    for (int i = 0; i < K1 * K1 / 2; ++i) wp[i] = bits16<T>(w[2 * i]) | (bits16<T>(w[2 * i + 1]) << 16);
 }
 
 // This pixel's weights for source row y, positions [x, x + NPOS): window row y - Y0 (nothing when the row is outside the
-// window), stored as bf16 at base + e * stride for position x + e.  The zero entries are the caller's to write.
+// window), stored as 16-bit values at base + e * stride for position x + e.  The zero entries are the caller's to write.
 template <int K, int NPOS = SEG>
 __device__ __forceinline__ void scatter_window_row(uint32_t base, uint32_t stride, const uint32_t (&wp)[(K + 1) * (K + 1) / 2],
                                                    int X0, int Y0, int y, int x) {
-    constexpr int K1 = K + 1, RW = K1 / 2;   // bf16 pairs per window row
+    constexpr int K1 = K + 1, RW = K1 / 2;   // 16-bit pairs per window row
     const int rr = y - Y0;
     if (rr < 0 || rr > K) return;
     uint32_t wr[RW];
@@ -165,21 +166,21 @@ __device__ __forceinline__ uint32_t warp_row_bits(bool active) {
 // followed by base_function.py:804-810).  One such pixel costs 4*k*k*C dependent loads, so a whole warp shares it:
 // every lane evaluates the (identical) softmax and taps, lanes split the channels.  The (i, j) loops stay rolled: an
 // unrolled tap table is register-hungry and would raise the pressure of (or spill into) the hot epilogue loop.
-template <int K, bool NHWC>
-__device__ __forceinline__ void irregular_pixel(const __nv_bfloat16* __restrict__ src, const __nv_bfloat16* __restrict__ logits,
-                                                __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ prev,
-                                                const __nv_bfloat16* __restrict__ mask, int b, int C, int Hs, int Ws, int H, int W,
+template <typename T, int K, bool NHWC>
+__device__ __forceinline__ void irregular_pixel(const T* __restrict__ src, const T* __restrict__ logits, T* __restrict__ out,
+                                                const T* __restrict__ prev, const T* __restrict__ mask, int b, int C, int Hs, int Ws,
+                                                int H, int W,
                                                 int qx, int qy, float qfx, float qfy, int lane) {
     constexpr int KK = K * K;
     const long long hw = (long long)H * W, qofs = (long long)qy * W + qx;
     float p[KK];
-    pixel_softmax<__nv_bfloat16, float, KK>(logits + (long long)b * KK * hw + qofs, hw, KK, p);   // every lane: same loads
+    pixel_softmax<T, float, KK>(logits + (long long)b * KK * hw + qofs, hw, KK, p);   // every lane: same loads
     const long long spl = (long long)Hs * Ws;
     const long long sc = NHWC ? 1 : spl, sp = NHWC ? C : 1;     // element strides: channel, position
-    const __nv_bfloat16* sb = src + (long long)b * spl * C;
-    __nv_bfloat16* ob = NHWC ? out + ((long long)b * hw + qofs) * C : out + (long long)b * C * hw + qofs;
+    const T* sb = src + (long long)b * spl * C;
+    T* ob = NHWC ? out + ((long long)b * hw + qofs) * C : out + (long long)b * C * hw + qofs;
     for (int c = lane; c < C; c += 32) {
-        const __nv_bfloat16* s = sb + c * sc;
+        const T* s = sb + c * sc;
         float acc = 0.f;
 #pragma unroll 1
         for (int i = 0; i < K; ++i) {      // rolled on purpose (rare path): keeps the tap table out of the registers
@@ -192,11 +193,11 @@ __device__ __forceinline__ void irregular_pixel(const __nv_bfloat16* __restrict_
         }
         acc *= 1.0f / static_cast<float>(KK);
         if (prev != nullptr) {
-            const float qm = __bfloat162float(mask[(long long)b * hw + qofs]);
-            const __nv_bfloat16* pb = NHWC ? prev + ((long long)b * hw + qofs) * C : prev + (long long)b * C * hw + qofs;
-            acc = __bfloat162float(pb[NHWC ? (long long)c : (long long)c * hw]) * (1.f - qm) + acc * qm;
+            const float qm = ld(mask + (long long)b * hw + qofs);
+            const T* pb = NHWC ? prev + ((long long)b * hw + qofs) * C : prev + (long long)b * C * hw + qofs;
+            acc = ld(pb + (NHWC ? (long long)c : (long long)c * hw)) * (1.f - qm) + acc * qm;
         }
-        ob[NHWC ? (long long)c : (long long)c * hw] = __float2bfloat16_rn(acc);
+        st(ob + (NHWC ? (long long)c : (long long)c * hw), acc);
     }
 }
 

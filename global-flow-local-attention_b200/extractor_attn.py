@@ -27,6 +27,16 @@ from .block_extractor import BlockExtractor
 from .local_attn_reshape import LocalAttnReshape
 
 
+def autocast_16(*ts):
+    """The autocast policy of the fused ops.  Under torch.autocast("cuda"), each floating-point tensor cast to the autocast
+    dtype, fp64 left alone (as torch's own autocast leaves it); outside autocast, the tensors as given.  Callers cast before
+    Function.apply, so autograd hands every gradient back in its input's own dtype."""
+    if not torch.is_autocast_enabled("cuda"):
+        return ts
+    dt = torch.get_autocast_dtype("cuda")
+    return tuple(t.to(dt) if t.is_floating_point() and t.dtype != torch.float64 else t for t in ts)
+
+
 class LocalAttnFunction(Function):
     """(source [B,C,Hs,Ws], flow [B,2,H,W], logits [B,k*k,H,W]) -> out [B,C,H,W]
 
@@ -34,6 +44,7 @@ class LocalAttnFunction(Function):
     """
 
     @staticmethod
+    @torch.amp.custom_fwd(device_type="cuda")
     def forward(ctx, source, flow_field, logits, kernel_size, algo="auto"):
         assert flow_field.is_contiguous() and logits.is_contiguous()
         ctx.save_for_backward(source, flow_field, logits)
@@ -42,6 +53,7 @@ class LocalAttnFunction(Function):
         return F_.local_attn_fwd(source, flow_field, logits, kernel_size, algo=algo)
 
     @staticmethod
+    @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, grad_output):
         source, flow_field, logits = ctx.saved_tensors
         gs, gf, gl = F_.local_attn_bwd(source, flow_field, logits, grad_output, ctx.kernel_size, algo=ctx.algo)
@@ -56,6 +68,8 @@ def _keep_format(t):
 
 
 def local_attention(source, flow_field, logits, kernel_size, algo="auto"):
+    """Under torch.autocast("cuda"), source and logits run in the autocast dtype (autocast_16) and the flow in fp32."""
+    source, logits = autocast_16(source, logits)
     return LocalAttnFunction.apply(_keep_format(source), F_.flow_f32(source, flow_field).contiguous(), logits.contiguous(),
                                    kernel_size, algo)
 
@@ -83,7 +97,10 @@ class PatchConvFunction(Function):
 def patch_conv(source, flow_field, weight, kernel_size):
     """conv2d(BlockExtractor(kernel_size)(source, flow_field), weight, None, stride=kernel_size): the source half of
     ExtractorAttn's first conv (base_function.py:800,805,807).  The kernels serve bf16 sources (channels-last, or NCHW
-    re-laid), C % 64 == 0 and 128 output channels; every other call runs that literal composition."""
+    re-laid), C % 64 == 0 and 128 output channels; every other call runs that literal composition.  Under
+    torch.autocast("cuda"), source and weight are cast to the autocast dtype first: bf16 then reaches the kernels, fp16
+    runs the composition (materialising the block tensor) as an fp16 call does outside autocast."""
+    source, weight = autocast_16(source, weight)
     src = _keep_format(source)
     flow32 = F_.flow_f32(src, flow_field).contiguous()
     if F_.patch_conv_eligible(src, flow32, weight, kernel_size):
@@ -145,10 +162,11 @@ class ExtractorAttn(nn.Module):
             if needs_grad:
                 out_attn = local_attention(source, flow_field, logits, self.kernel_size)
                 return target * (1 - mask) + out_attn * mask
-            src = _keep_format(source)
+            # under autocast, the attention's dtype is the autocast dtype: target and mask follow it
+            src, logits, target = autocast_16(_keep_format(source), logits, target)
             fmt = torch.channels_last if (not src.is_contiguous()) else torch.contiguous_format
             return F_.local_attn_blend_fwd(src, F_.flow_f32(src, flow_field).contiguous(), logits.contiguous(),
-                                           target.contiguous(memory_format=fmt), mask.to(source.dtype), self.kernel_size)
+                                           target.contiguous(memory_format=fmt), mask.to(src.dtype), self.kernel_size)
         assert mask is None, "mask blend is only fused for the softmax variant"
         # softmax=None in the reference means "apply the nonlinearity instead": keep the literal composition
         attn_param = self.reshape(self.fully_connect_layer[-1](logits), self.kernel_size)
@@ -157,6 +175,7 @@ class ExtractorAttn(nn.Module):
     def hook_attn_param(self, source, target, flow_field):
         logits, block_source = self._logits(source, target, flow_field, materialise=not self.fused_softmax)
         if self.fused_softmax:
+            source, logits = autocast_16(source, logits)
             result, probs = F_.local_attn_fwd(_keep_format(source), F_.flow_f32(source, flow_field).contiguous(), logits.contiguous(),
                                               self.kernel_size, return_probs=True)
             return probs, result

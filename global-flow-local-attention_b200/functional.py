@@ -480,7 +480,7 @@ def patch_conv_bwd(source, flow, weight, grad_out, k):
 def _tile_bwd_eligible(source, flow, k) -> bool:
     """what the backward tile kernels serve (mirrors local_attn_bwd_tc_supported in csrc/local_attn_bwd_tc.cu)"""
     c = source.shape[1]
-    return (source.dtype == torch.bfloat16 and flow.dtype == torch.float32 and k in (3, 5)
+    return (source.dtype in _HALF and flow.dtype == torch.float32 and k in (3, 5)
             and (c % 256 == 0 or c in (64, 128)))
 
 

@@ -85,7 +85,7 @@ int gfla_debug_wait_profile(int which, int enable, unsigned long long* out_u64x6
 
 /* Re-layout of a [B,C,H,W] feature tensor between planar NCHW and channels-last NHWC storage
  * (out of place; to_nhwc = 1: NCHW -> NHWC, 0: NHWC -> NCHW).  Not part of the reference's API: the
- * Python layer uses it to serve planar bf16 callers with the channels-last tile kernels. */
+ * Python layer uses it to serve planar bf16 / fp16 callers with the channels-last tile kernels. */
 int gfla_relayout(const void* src, void* dst, int B, int C, int H, int W, int dtype, int to_nhwc,
                   gfla_stream_t stream);
 

@@ -344,3 +344,70 @@ if "resample16" in which:   # resample2d and the fused resample2d -> cosine on b
                           "peak_extra_MB": round((torch.cuda.max_memory_allocated() - base) / 2 ** 20, 1)}), flush=True)
         del vgg, imgs, flows, loss_fn
         torch.cuda.empty_cache()
+
+if "fp16" in which:   # fp16 local attention: (a) the fp16 tile kernels, (b) bf16 on the same kernels, (c) fp16 as it ran before
+    # the fp16 tile instances (the gather forward, the backward on fp32 copies), alternated in one process; then one
+    # PoseGenerator training step (fp32 weights, channels-last) under autocast fp16, autocast bf16 and in plain fp32
+    import statistics
+    import subprocess
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+    card = q.stdout.strip() or torch.cuda.get_device_name(0)
+    cl = torch.channels_last
+    med = lambda v: round(statistics.median(v), 4)
+    ARMS = {"a fp16 tile": (torch.float16, "auto"), "b bf16 tile": (torch.bfloat16, "auto"), "c fp16 gather / fp32 copies": (torch.float16, "gather")}
+    for (B, C, HW, k, flows) in ((16, 256, 256, 5, ("smooth", "iid")), (8, 256, 32, 3, ("smooth",)), (8, 128, 64, 5, ("smooth",))):
+        for fname in flows:
+            flow = smooth(B, HW, HW) if fname == "smooth" else (torch.rand(B, 2, HW, HW, device=dev) * 8 - 4)
+            base = [torch.randn(B, C, HW, HW, device=dev), torch.randn(B, k * k, HW, HW, device=dev), torch.randn(B, C, HW, HW, device=dev)]
+            data = {}
+            for arm, (dt, algo) in ARMS.items():
+                s_, l_, g_ = base[0].to(dt).contiguous(memory_format=cl), base[1].to(dt), base[2].to(dt).contiguous(memory_format=cl)
+                data[arm] = (s_, l_, g_, algo)
+            del base
+            res = {arm: {"fwd": [], "bwd": [], "step": []} for arm in ARMS}
+            for _ in range(5):
+                for arm, (s_, l_, g_, algo) in data.items():
+                    n, w = (2, 1) if algo == "gather" and B * HW * HW > 2 ** 20 else (5, 2)
+                    fwd = lambda: F_.local_attn_fwd(s_, flow, l_, k, algo=algo)
+                    bwd = lambda: F_.local_attn_bwd(s_, flow, l_, g_, k, algo=algo)
+                    res[arm]["fwd"].append(timed(fwd, n=n, w=w))
+                    res[arm]["bwd"].append(timed(bwd, n=n, w=w))
+                    res[arm]["step"].append(timed(lambda: (fwd(), bwd()), n=n, w=w))
+            print(json.dumps({"op": "local attention fwd / bwd / step by dtype",
+                              "config": f"B={B} C={C} {HW}x{HW} k={k} channels_last, {fname} flow (fp32)",
+                              **{f"{part}_ms": {arm: med(res[arm][part]) for arm in ARMS} for part in ("fwd", "bwd", "step")},
+                              "step_ms_all": {arm: [round(v, 4) for v in res[arm]["step"]] for arm in ARMS},
+                              "card_and_power_limit": card,
+                              "timing": "CUDA events, median of 5 alternating rounds (5 calls after 2 warm-up; 2 after 1 for arm c at cfg2)"}),
+                  flush=True)
+            del data, flow
+            torch.cuda.empty_cache()
+    import bench_models
+    if bench_models.reference_root() is None:
+        print(json.dumps({"op": "PoseGenerator step by precision", "skipped": "baseline/_ref snapshot of the reference generators missing"}))
+    else:
+        Pose, _ = bench_models.load_generators("fused")
+        torch.manual_seed(11)
+        net = Pose(**bench_models.POSE_KW)
+        net.init_weights("orthogonal", gain=0.5)
+        net = net.to(dev).to(memory_format=cl)
+        gen = torch.Generator(device="cpu").manual_seed(3)
+        x = [torch.randn(4, c, 256, 256, generator=gen).to(dev).contiguous(memory_format=cl) for c in (3, 18, 18)]
+        tf32 = {"cudnn.allow_tf32": torch.backends.cudnn.allow_tf32, "cuda.matmul.allow_tf32": torch.backends.cuda.matmul.allow_tf32}
+
+        def train_step(dt):
+            net.zero_grad(set_to_none=True)
+            with torch.autocast("cuda", dtype=dt or torch.float32, enabled=dt is not None):
+                img, flows, _ = net(*x)
+                loss = img.float().mean() + sum(f.float().pow(2).mean() for f in flows)
+            loss.backward()
+        parms = {"autocast fp16": torch.float16, "autocast bf16": torch.bfloat16, "fp32": None}
+        pres = {a: [] for a in parms}
+        for _ in range(5):
+            for a, dt in parms.items():
+                pres[a].append(timed(lambda: train_step(dt), n=3, w=1))
+        print(json.dumps({"op": "PoseGenerator forward+backward by precision (fp32 weights, channels_last)",
+                          "config": "B=4 256x256, POSE_KW of bench_models, fused ExtractorAttn",
+                          "ms": {a: med(v) for a, v in pres.items()}, "ms_all": {a: [round(t, 2) for t in v] for a, v in pres.items()},
+                          "tf32_state_of_the_fp32_arm": tf32, "card_and_power_limit": card,
+                          "timing": "CUDA events, median of 5 alternating rounds of 3 steps after 1 warm-up"}), flush=True)
