@@ -15,7 +15,6 @@
 import sys
 import types
 
-from . import _lib
 from . import functional as F_
 
 
@@ -30,9 +29,8 @@ def _be_forward(source, flow_field, output, kernel_size):
     F_._need_cuda(source, flow_field, output)
     b, c, hs, ws = source.shape
     _, _, hf, wf = flow_field.shape
-    _lib.check(_lib.lib().gfla_block_extract_fwd(source.data_ptr(), flow_field.data_ptr(), output.data_ptr(), b, c, hs,
-                                                 ws, hf, wf, kernel_size, F_._dt(source), F_._dt(flow_field),
-                                                 F_._stream(source)), "block_extractor_cuda.forward")
+    F_._call("block_extract_fwd", source, source.data_ptr(), flow_field.data_ptr(), output.data_ptr(), b, c, hs, ws, hf, wf,
+             kernel_size, F_._dt(source), F_._dt(flow_field))
     return 1
 
 
@@ -44,8 +42,7 @@ def _be_backward(source, flow_field, grad_output, grad_source, grad_flow_field, 
 def _lr_forward(inputs, output, kernel_size):
     F_._need_cuda(inputs, output)
     b, _, h, w = inputs.shape
-    _lib.check(_lib.lib().gfla_attn_reshape_fwd(inputs.data_ptr(), output.data_ptr(), b, h, w, kernel_size,
-                                                F_._dt(inputs), F_._stream(inputs)), "local_attn_reshape_cuda.forward")
+    F_._call("attn_reshape_fwd", inputs, inputs.data_ptr(), output.data_ptr(), b, h, w, kernel_size, F_._dt(inputs))
     return 1
 
 
@@ -58,9 +55,8 @@ def _rs_forward(input1, input2, output, kernel_size, dilation):
     F_._need_cuda(input1, input2, output)
     _, c, hi, wi = input1.shape
     b, _, h, w = input2.shape
-    _lib.check(_lib.lib().gfla_resample2d_fwd(input1.data_ptr(), input2.data_ptr(), output.data_ptr(), b, c, hi, wi, h,
-                                              w, kernel_size, dilation, F_._dt(input1), F_._stream(input1)),
-               "resample2d_cuda.forward")
+    F_._call("resample2d_fwd", input1, input1.data_ptr(), input2.data_ptr(), output.data_ptr(), b, c, hi, wi, h, w, kernel_size,
+             dilation, F_._dt(input1))
     return 1
 
 

@@ -1,5 +1,5 @@
-// extern "C" surface of libgfla_warp.so (declared in include/gfla_warp.h):
-// argument validation + dispatch; no state, no allocation.
+// extern "C" surface of libgfla_warp.so (declared in include/gfla_warp.h): argument validation + dispatch, and the
+// process-wide launch counter.
 #include "det_accum.cuh"
 
 namespace gfla {
@@ -35,6 +35,7 @@ int patch_conv_bwd_det(const void*, const void*, const void*, const void*, void*
 }  // namespace gfla
 
 #include <atomic>
+#include <initializer_list>
 
 namespace gfla {
 static std::atomic<unsigned long long> g_launches{0};
@@ -45,9 +46,95 @@ using namespace gfla;
 
 #define REQ_PTR(p) do { if ((p) == nullptr) return GFLA_E_NULL; } while (0)
 #define REQ_ALIGN(p, dt) do { if (!aligned((p), elem_size(dt))) return GFLA_E_ALIGN; } while (0)
+#define REQ_OK(expr) do { const int r_ = (expr); if (r_ != GFLA_OK) return r_; } while (0)
 
-static inline bool pos(int a) { return a > 0; }
+template <typename... I> static inline bool pos(I... sizes) { return ((sizes > 0) && ...); }
+static inline bool k_ok(int k) { return k >= 1 && k <= 9; }
 static inline bool dtype_known(int d) { return elem_size(d) != 0; }
+
+// every non-NULL pointer aligned to dtype's element size (NULL: an optional buffer the caller left out)
+static inline bool all_aligned(std::initializer_list<const void*> ps, int dtype) {
+    for (const void* p : ps)
+        if (p != nullptr && !aligned(p, elem_size(dtype))) return false;
+    return true;
+}
+
+// The two resample2d families: F32 / F64 with every buffer in dtype (half = false), or BF16 / F16 feature maps (`data`)
+// next to an fp32 flow, stats, grad_in2, grad_in1 and grad_val (`wide`, half = true).  eps: 0 for the plain ops.
+static int resample2d_args(bool half, int B, int C, int Hi, int Wi, int H, int W, int ks, int dilation, double eps, int dtype,
+                           std::initializer_list<const void*> data, std::initializer_list<const void*> wide) {
+    if (!pos(B, C, Hi, Wi, H, W) || ks < 2 || ks > 9 || dilation < 1 || !(eps >= 0)) return GFLA_E_SHAPE;
+    if (half ? (dtype != GFLA_BF16 && dtype != GFLA_F16) : (dtype != GFLA_F32 && dtype != GFLA_F64)) return GFLA_E_DTYPE;
+    if (!all_aligned(data, dtype) || !all_aligned(wide, half ? GFLA_F32 : dtype)) return GFLA_E_ALIGN;
+    return GFLA_OK;
+}
+
+// Layout, shape, dtype and algo checks of the local-attention entry points, and the alignment of their buffers (`data` in
+// dtype, `flows` in flow_dtype).  The caller has checked its required pointers.
+static int local_attn_args(int B, int C, int Hs, int Ws, int H, int W, int k, int dtype, int flow_dtype, int layout, int algo,
+                           std::initializer_list<const void*> data, std::initializer_list<const void*> flows) {
+    if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
+    if (!pos(B, C, Hs, Ws, H, W) || !k_ok(k)) return GFLA_E_SHAPE;
+    if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
+    if (algo < 0 || algo > 2) return GFLA_E_NOTSUP;
+    if (!all_aligned(data, dtype) || !all_aligned(flows, flow_dtype)) return GFLA_E_ALIGN;
+    return GFLA_OK;
+}
+
+// the two local-attention backward passes check the layout before the pointers
+static int local_attn_bwd_args(const void* source, const void* flow, const void* logits, const void* grad_out, const void* grad_source,
+                               const void* grad_flow, const void* grad_logits, int B, int C, int Hs, int Ws, int H, int W, int k,
+                               int dtype, int flow_dtype, int layout, int algo) {
+    if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
+    REQ_PTR(source); REQ_PTR(flow); REQ_PTR(logits); REQ_PTR(grad_out); REQ_PTR(grad_source); REQ_PTR(grad_flow); REQ_PTR(grad_logits);
+    return local_attn_args(B, C, Hs, Ws, H, W, k, dtype, flow_dtype, layout, algo, {source, logits, grad_out, grad_source, grad_logits},
+                           {flow, grad_flow});
+}
+
+// shape, dtype and support checks shared by the patch-convolution entry points
+static int patch_conv_args(int B, int C, int Hs, int Ws, int H, int W, int k, int N, int dtype, int flow_dtype, int layout) {
+    if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
+    if (!pos(B, C, Hs, Ws, H, W, N) || !k_ok(k)) return GFLA_E_SHAPE;
+    if (dtype != GFLA_BF16 || flow_dtype != GFLA_F32) return GFLA_E_DTYPE;
+    if (!patch_conv_supported(C, N, dtype, flow_dtype, layout)) return GFLA_E_NOTSUP;
+    return GFLA_OK;
+}
+
+// ------------------------------------------------------------------ deterministic backward passes (det_accum.cuh)
+// The workspace of each: the fixed-point sums of every scattered output, the exponents and the maxima (fx_layout).
+// Local attention and block_extractor scatter grad_source [B][C][Hs][Ws] only, with one exponent and maximum per image.
+static FxLayout scatter_det_layout(int B, int C, int Hs, int Ws) { return fx_layout((long long)B * C * Hs * Ws, B, B); }
+static FxLayout pc_det_layout(int B, int C, int Hs, int Ws, int k, int N) {
+    return fx_layout((long long)B * Hs * Ws * C + (long long)N * k * k * C, B + 1, B + 2);
+}
+
+// NULL workspace: GFLA_E_NULL; not 16-byte aligned: GFLA_E_ALIGN; smaller than needed: GFLA_E_SHAPE
+static int ws_check(const void* ws, long long bytes, const FxLayout& l) {
+    if (ws == nullptr) return GFLA_E_NULL;
+    if (!aligned(ws, 16)) return GFLA_E_ALIGN;
+    if (bytes < 0 || (size_t)bytes < l.total) return GFLA_E_SHAPE;
+    return GFLA_OK;
+}
+
+#define FX_PARTS(ws, l) \
+    fx_t* sums = reinterpret_cast<fx_t*>(ws); \
+    int* exps = reinterpret_cast<int*>(static_cast<char*>(ws) + (l).exps); \
+    fx_t* amax = reinterpret_cast<fx_t*>(static_cast<char*>(ws) + (l).amax)
+
+// The deterministic backward of an op that scatters only grad_source (a checked scatter_det_layout workspace): zero the
+// workspace, max|G_b| over the gout_per_image elements of each image of grad_out, E_b from the bound factor * max|G_b|,
+// the scatter kernel(sums, exps), and one narrowing pass into grad_source.
+template <typename Kernel>
+static int det_scatter(void* workspace, const FxLayout& l, const void* grad_out, long long gout_per_image, double factor,
+                       void* grad_source, long long src_per_image, int B, int dtype, int accumulate, cudaStream_t st_, Kernel&& kernel) {
+    FX_PARTS(workspace, l);
+    int r = zero_async(workspace, l.total, st_);
+    if (r == GFLA_OK) r = fx_amax(grad_out, dtype, gout_per_image, B, amax, st_);
+    if (r == GFLA_OK) r = fx_exponents(amax, B, nullptr, factor, false, exps, st_);
+    if (r == GFLA_OK) r = kernel(sums, exps);
+    if (r == GFLA_OK) r = fx_narrow(sums, exps, src_per_image, B * src_per_image, grad_source, dtype, accumulate, st_);
+    return r;
+}
 
 extern "C" {
 
@@ -89,7 +176,7 @@ int gfla_debug_set_buffer(void* host_mapped_u64x8) {
 
 int gfla_relayout(const void* src, void* dst, int B, int C, int H, int W, int dtype, int to_nhwc, gfla_stream_t stream) {
     REQ_PTR(src); REQ_PTR(dst);
-    if (!pos(B) || !pos(C) || !pos(H) || !pos(W)) return GFLA_E_SHAPE;
+    if (!pos(B, C, H, W)) return GFLA_E_SHAPE;
     if (!dtype_known(dtype)) return GFLA_E_DTYPE;
     if (src == dst) return GFLA_E_NOTSUP;
     REQ_ALIGN(src, dtype); REQ_ALIGN(dst, dtype);
@@ -99,7 +186,7 @@ int gfla_relayout(const void* src, void* dst, int B, int C, int H, int W, int dt
 int gfla_block_extract_fwd(const void* source, const void* flow, void* out, int B, int C, int Hs, int Ws, int Hf,
                            int Wf, int k, int dtype, int flow_dtype, gfla_stream_t stream) {
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(out);
-    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(Hf) || !pos(Wf) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    if (!pos(B, C, Hs, Ws, Hf, Wf) || !k_ok(k)) return GFLA_E_SHAPE;
     if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
     REQ_ALIGN(source, dtype); REQ_ALIGN(out, dtype); REQ_ALIGN(flow, flow_dtype);
     return block_extract_fwd(source, flow, out, B, C, Hs, Ws, Hf, Wf, k, dtype, flow_dtype, (cudaStream_t)stream);
@@ -109,7 +196,7 @@ int gfla_block_extract_bwd(const void* source, const void* flow, const void* gra
                            void* grad_flow, int B, int C, int Hs, int Ws, int Hf, int Wf, int k, int dtype,
                            int flow_dtype, int grad_source_dtype, int accumulate, gfla_stream_t stream) {
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(grad_out); REQ_PTR(grad_source); REQ_PTR(grad_flow);
-    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(Hf) || !pos(Wf) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    if (!pos(B, C, Hs, Ws, Hf, Wf) || !k_ok(k)) return GFLA_E_SHAPE;
     if (!dtypes_ok(dtype, flow_dtype, grad_source_dtype)) return GFLA_E_DTYPE;
     REQ_ALIGN(source, dtype); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_source, grad_source_dtype);
     REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
@@ -127,7 +214,7 @@ int gfla_convert(const void* src, int src_dtype, void* dst, int dst_dtype, long 
 
 int gfla_attn_reshape_fwd(const void* in, void* out, int B, int H, int W, int k, int dtype, gfla_stream_t stream) {
     REQ_PTR(in); REQ_PTR(out);
-    if (!pos(B) || !pos(H) || !pos(W) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    if (!pos(B, H, W) || !k_ok(k)) return GFLA_E_SHAPE;
     if (!dtype_known(dtype)) return GFLA_E_DTYPE;
     REQ_ALIGN(in, dtype); REQ_ALIGN(out, dtype);
     return attn_reshape_fwd(in, out, B, H, W, k, dtype, (cudaStream_t)stream);
@@ -136,18 +223,17 @@ int gfla_attn_reshape_fwd(const void* in, void* out, int B, int H, int W, int k,
 int gfla_attn_reshape_bwd(const void* grad_out, void* grad_in, int B, int H, int W, int k, int dtype, int accumulate,
                           gfla_stream_t stream) {
     REQ_PTR(grad_out); REQ_PTR(grad_in);
-    if (!pos(B) || !pos(H) || !pos(W) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    if (!pos(B, H, W) || !k_ok(k)) return GFLA_E_SHAPE;
     if (!dtype_known(dtype)) return GFLA_E_DTYPE;
     REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_in, dtype);
     return attn_reshape_bwd(grad_out, grad_in, B, H, W, k, dtype, accumulate, (cudaStream_t)stream);
 }
 
+// ------------------------------------------------------------------ resample2d: the fp32 / fp64 and the 16-bit families
 int gfla_resample2d_fwd(const void* in1, const void* in2, void* out, int B, int C, int Hi, int Wi, int H, int W, int ks,
                         int dilation, int dtype, gfla_stream_t stream) {
     REQ_PTR(in1); REQ_PTR(in2); REQ_PTR(out);
-    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1) return GFLA_E_SHAPE;
-    if (dtype != GFLA_F32 && dtype != GFLA_F64) return GFLA_E_DTYPE;
-    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2, dtype); REQ_ALIGN(out, dtype);
+    REQ_OK(resample2d_args(false, B, C, Hi, Wi, H, W, ks, dilation, 0.0, dtype, {in1, out}, {in2}));
     return resample2d_fwd(in1, in2, out, B, C, Hi, Wi, H, W, ks, dilation, dtype, (cudaStream_t)stream);
 }
 
@@ -155,9 +241,7 @@ int gfla_resample2d_bwd(const void* in1, const void* in2, const void* grad_out, 
                         int C, int Hi, int Wi, int H, int W, int ks, int dilation, int dtype, int accumulate,
                         gfla_stream_t stream) {
     REQ_PTR(in1); REQ_PTR(in2); REQ_PTR(grad_out); REQ_PTR(grad_in1); REQ_PTR(grad_in2);
-    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1) return GFLA_E_SHAPE;
-    if (dtype != GFLA_F32 && dtype != GFLA_F64) return GFLA_E_DTYPE;
-    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2, dtype); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_in1, dtype); REQ_ALIGN(grad_in2, dtype);
+    REQ_OK(resample2d_args(false, B, C, Hi, Wi, H, W, ks, dilation, 0.0, dtype, {in1, grad_out}, {in2, grad_in1, grad_in2}));
     return resample2d_bwd(in1, in2, grad_out, grad_in1, grad_in2, B, C, Hi, Wi, H, W, ks, dilation, dtype, accumulate,
                           (cudaStream_t)stream);
 }
@@ -165,9 +249,7 @@ int gfla_resample2d_bwd(const void* in1, const void* in2, const void* grad_out, 
 int gfla_resample2d_cosine_fwd(const void* in1, const void* in2, const void* target, void* cos_out, void* stats, int B, int C, int Hi,
                                int Wi, int H, int W, int ks, int dilation, double eps, int dtype, gfla_stream_t stream) {
     REQ_PTR(in1); REQ_PTR(in2); REQ_PTR(target); REQ_PTR(cos_out); REQ_PTR(stats);
-    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1 || !(eps >= 0)) return GFLA_E_SHAPE;
-    if (dtype != GFLA_F32 && dtype != GFLA_F64) return GFLA_E_DTYPE;
-    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2, dtype); REQ_ALIGN(target, dtype); REQ_ALIGN(cos_out, dtype); REQ_ALIGN(stats, dtype);
+    REQ_OK(resample2d_args(false, B, C, Hi, Wi, H, W, ks, dilation, eps, dtype, {in1, target, cos_out}, {in2, stats}));
     return resample2d_cos_fwd(in1, in2, target, cos_out, stats, B, C, Hi, Wi, H, W, ks, dilation, eps, dtype, (cudaStream_t)stream);
 }
 
@@ -176,36 +258,23 @@ int gfla_resample2d_cosine_bwd(const void* in1, const void* in2, const void* tar
                                int W, int ks, int dilation, double eps, int dtype, int accumulate, gfla_stream_t stream) {
     REQ_PTR(in1); REQ_PTR(in2); REQ_PTR(target); REQ_PTR(stats); REQ_PTR(grad_cos); REQ_PTR(grad_in2);
     if (grad_in1 != nullptr && grad_val == nullptr) return GFLA_E_NULL;      // the scatter runs on the materialised d/d(warped)
-    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1 || !(eps >= 0)) return GFLA_E_SHAPE;
-    if (dtype != GFLA_F32 && dtype != GFLA_F64) return GFLA_E_DTYPE;
-    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2, dtype); REQ_ALIGN(target, dtype); REQ_ALIGN(stats, dtype); REQ_ALIGN(grad_cos, dtype);
-    REQ_ALIGN(grad_in2, dtype);
-    if (grad_in1 != nullptr) { REQ_ALIGN(grad_in1, dtype); }
-    if (grad_val != nullptr) { REQ_ALIGN(grad_val, dtype); }
-    if (grad_target != nullptr) { REQ_ALIGN(grad_target, dtype); }
+    REQ_OK(resample2d_args(false, B, C, Hi, Wi, H, W, ks, dilation, eps, dtype, {in1, target, grad_cos, grad_target},
+                           {in2, stats, grad_in2, grad_in1, grad_val}));
     return resample2d_cos_bwd(in1, in2, target, stats, grad_cos, grad_in1, grad_in2, grad_val, grad_target, B, C, Hi, Wi, H, W, ks, dilation,
                               eps, dtype, accumulate, (cudaStream_t)stream);
 }
 
-// 16-bit storage: the feature maps in dtype (BF16 / F16 only), the flow, stats, grad_in2, grad_in1 and grad_val in fp32
-static inline bool dtype16(int d) { return d == GFLA_BF16 || d == GFLA_F16; }
-
 int gfla_resample2d16_fwd(const void* in1, const void* in2_f32, void* out, int B, int C, int Hi, int Wi, int H, int W, int ks,
                           int dilation, int dtype, gfla_stream_t stream) {
     REQ_PTR(in1); REQ_PTR(in2_f32); REQ_PTR(out);
-    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1) return GFLA_E_SHAPE;
-    if (!dtype16(dtype)) return GFLA_E_DTYPE;
-    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2_f32, GFLA_F32); REQ_ALIGN(out, dtype);
+    REQ_OK(resample2d_args(true, B, C, Hi, Wi, H, W, ks, dilation, 0.0, dtype, {in1, out}, {in2_f32}));
     return resample2d_fwd(in1, in2_f32, out, B, C, Hi, Wi, H, W, ks, dilation, dtype, (cudaStream_t)stream);
 }
 
 int gfla_resample2d16_bwd(const void* in1, const void* in2_f32, const void* grad_out, void* grad_in1_f32, void* grad_in2_f32, int B,
                           int C, int Hi, int Wi, int H, int W, int ks, int dilation, int dtype, int accumulate, gfla_stream_t stream) {
     REQ_PTR(in1); REQ_PTR(in2_f32); REQ_PTR(grad_out); REQ_PTR(grad_in1_f32); REQ_PTR(grad_in2_f32);
-    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1) return GFLA_E_SHAPE;
-    if (!dtype16(dtype)) return GFLA_E_DTYPE;
-    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2_f32, GFLA_F32); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_in1_f32, GFLA_F32);
-    REQ_ALIGN(grad_in2_f32, GFLA_F32);
+    REQ_OK(resample2d_args(true, B, C, Hi, Wi, H, W, ks, dilation, 0.0, dtype, {in1, grad_out}, {in2_f32, grad_in1_f32, grad_in2_f32}));
     return resample2d_bwd(in1, in2_f32, grad_out, grad_in1_f32, grad_in2_f32, B, C, Hi, Wi, H, W, ks, dilation, dtype, accumulate,
                           (cudaStream_t)stream);
 }
@@ -213,9 +282,7 @@ int gfla_resample2d16_bwd(const void* in1, const void* in2_f32, const void* grad
 int gfla_resample2d16_cosine_fwd(const void* in1, const void* in2_f32, const void* target, void* cos_out, void* stats_f32, int B, int C,
                                  int Hi, int Wi, int H, int W, int ks, int dilation, double eps, int dtype, gfla_stream_t stream) {
     REQ_PTR(in1); REQ_PTR(in2_f32); REQ_PTR(target); REQ_PTR(cos_out); REQ_PTR(stats_f32);
-    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1 || !(eps >= 0)) return GFLA_E_SHAPE;
-    if (!dtype16(dtype)) return GFLA_E_DTYPE;
-    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2_f32, GFLA_F32); REQ_ALIGN(target, dtype); REQ_ALIGN(cos_out, dtype); REQ_ALIGN(stats_f32, GFLA_F32);
+    REQ_OK(resample2d_args(true, B, C, Hi, Wi, H, W, ks, dilation, eps, dtype, {in1, target, cos_out}, {in2_f32, stats_f32}));
     return resample2d_cos_fwd(in1, in2_f32, target, cos_out, stats_f32, B, C, Hi, Wi, H, W, ks, dilation, eps, dtype, (cudaStream_t)stream);
 }
 
@@ -224,28 +291,18 @@ int gfla_resample2d16_cosine_bwd(const void* in1, const void* in2_f32, const voi
                                  int H, int W, int ks, int dilation, double eps, int dtype, int accumulate, gfla_stream_t stream) {
     REQ_PTR(in1); REQ_PTR(in2_f32); REQ_PTR(target); REQ_PTR(stats_f32); REQ_PTR(grad_cos); REQ_PTR(grad_in2_f32);
     if (grad_in1_f32 != nullptr && grad_val_f32 == nullptr) return GFLA_E_NULL;
-    if (!pos(B) || !pos(C) || !pos(Hi) || !pos(Wi) || !pos(H) || !pos(W) || ks < 2 || ks > 9 || dilation < 1 || !(eps >= 0)) return GFLA_E_SHAPE;
-    if (!dtype16(dtype)) return GFLA_E_DTYPE;
-    REQ_ALIGN(in1, dtype); REQ_ALIGN(in2_f32, GFLA_F32); REQ_ALIGN(target, dtype); REQ_ALIGN(stats_f32, GFLA_F32); REQ_ALIGN(grad_cos, dtype);
-    REQ_ALIGN(grad_in2_f32, GFLA_F32);
-    if (grad_in1_f32 != nullptr) { REQ_ALIGN(grad_in1_f32, GFLA_F32); }
-    if (grad_val_f32 != nullptr) { REQ_ALIGN(grad_val_f32, GFLA_F32); }
-    if (grad_target != nullptr) { REQ_ALIGN(grad_target, dtype); }
+    REQ_OK(resample2d_args(true, B, C, Hi, Wi, H, W, ks, dilation, eps, dtype, {in1, target, grad_cos, grad_target},
+                           {in2_f32, stats_f32, grad_in2_f32, grad_in1_f32, grad_val_f32}));
     return resample2d_cos_bwd(in1, in2_f32, target, stats_f32, grad_cos, grad_in1_f32, grad_in2_f32, grad_val_f32, grad_target, B, C, Hi, Wi,
                               H, W, ks, dilation, eps, dtype, accumulate, (cudaStream_t)stream);
 }
 
+// ------------------------------------------------------------------ local attention
 static int local_attn_fwd_any(const void* source, const void* flow, const void* logits, void* out, void* probs,
                               const void* prev, const void* mask, int B, int C, int Hs, int Ws, int H, int W, int k, int dtype,
                               int flow_dtype, int layout, int algo, gfla_stream_t stream) {
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(logits); REQ_PTR(out);
-    if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
-    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || k < 1 || k > 9) return GFLA_E_SHAPE;
-    if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
-    if (algo < 0 || algo > 2) return GFLA_E_NOTSUP;
-    REQ_ALIGN(source, dtype); REQ_ALIGN(logits, dtype); REQ_ALIGN(out, dtype); REQ_ALIGN(flow, flow_dtype);
-    if (probs) REQ_ALIGN(probs, dtype);
-    if (prev) { REQ_ALIGN(prev, dtype); REQ_ALIGN(mask, dtype); }
+    REQ_OK(local_attn_args(B, C, Hs, Ws, H, W, k, dtype, flow_dtype, layout, algo, {source, logits, out, probs, prev, mask}, {flow}));
     const bool tc_ok = local_attn_fwd_tc_supported(C, Ws, k, dtype, flow_dtype, layout, source, out) &&
                        (prev == nullptr || layout == GFLA_NCHW || aligned(prev, 16));
     if (algo == 2 && !tc_ok) return GFLA_E_NOTSUP;
@@ -272,13 +329,8 @@ int gfla_local_attn_blend_fwd(const void* source, const void* flow, const void* 
 int gfla_local_attn_bwd(const void* source, const void* flow, const void* logits, const void* grad_out,
                         void* grad_source, void* grad_flow, void* grad_logits, int B, int C, int Hs, int Ws, int H, int W,
                         int k, int dtype, int flow_dtype, int layout, int accumulate, int algo, gfla_stream_t stream) {
-    if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
-    REQ_PTR(source); REQ_PTR(flow); REQ_PTR(logits); REQ_PTR(grad_out); REQ_PTR(grad_source); REQ_PTR(grad_flow); REQ_PTR(grad_logits);
-    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || k < 1 || k > 9) return GFLA_E_SHAPE;
-    if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
-    if (algo < 0 || algo > 2) return GFLA_E_NOTSUP;
-    REQ_ALIGN(source, dtype); REQ_ALIGN(logits, dtype); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_source, dtype);
-    REQ_ALIGN(grad_logits, dtype); REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
+    REQ_OK(local_attn_bwd_args(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype,
+                               flow_dtype, layout, algo));
     const bool tc_ok = local_attn_bwd_tc_supported(C, k, dtype, flow_dtype, layout, source, grad_out, grad_source);
     if (algo == 2 && !tc_ok) return GFLA_E_NOTSUP;
     if (algo == 2 || (algo == 0 && tc_ok))
@@ -288,20 +340,11 @@ int gfla_local_attn_bwd(const void* source, const void* flow, const void* logits
                                  k, dtype, flow_dtype, accumulate, layout, (cudaStream_t)stream);
 }
 
-// shape, dtype and support checks shared by the two patch-convolution entry points
-static int patch_conv_args(int B, int C, int Hs, int Ws, int H, int W, int k, int N, int dtype, int flow_dtype, int layout) {
-    if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
-    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || !pos(N) || k < 1 || k > 9) return GFLA_E_SHAPE;
-    if (dtype != GFLA_BF16 || flow_dtype != GFLA_F32) return GFLA_E_DTYPE;
-    if (!patch_conv_supported(C, N, dtype, flow_dtype, layout)) return GFLA_E_NOTSUP;
-    return GFLA_OK;
-}
-
+// ------------------------------------------------------------------ patch convolution
 int gfla_patch_conv_fwd(const void* source, const void* flow, const void* weight, void* out, int B, int C, int Hs, int Ws, int H,
                         int W, int k, int N, int dtype, int flow_dtype, int layout, gfla_stream_t stream) {
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(weight); REQ_PTR(out);
-    const int e = patch_conv_args(B, C, Hs, Ws, H, W, k, N, dtype, flow_dtype, layout);
-    if (e != GFLA_OK) return e;
+    REQ_OK(patch_conv_args(B, C, Hs, Ws, H, W, k, N, dtype, flow_dtype, layout));
     if (!aligned(source, 16) || !aligned(weight, 16) || !aligned(out, 16)) return GFLA_E_ALIGN;
     REQ_ALIGN(flow, flow_dtype);
     return patch_conv_fwd(source, flow, weight, out, B, C, Hs, Ws, H, W, k, (cudaStream_t)stream);
@@ -312,8 +355,7 @@ int gfla_patch_conv_bwd(const void* source, const void* flow, const void* weight
                         int flow_dtype, int layout, int accumulate, gfla_stream_t stream) {
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(weight); REQ_PTR(grad_out);
     REQ_PTR(grad_source_f32); REQ_PTR(grad_flow); REQ_PTR(grad_weight_f32);
-    const int e = patch_conv_args(B, C, Hs, Ws, H, W, k, N, dtype, flow_dtype, layout);
-    if (e != GFLA_OK) return e;
+    REQ_OK(patch_conv_args(B, C, Hs, Ws, H, W, k, N, dtype, flow_dtype, layout));
     if (!aligned(source, 16) || !aligned(weight, 16) || !aligned(grad_out, 16) || !aligned(grad_source_f32, 16) ||
         !aligned(grad_weight_f32, 16))
         return GFLA_E_ALIGN;
@@ -322,53 +364,25 @@ int gfla_patch_conv_bwd(const void* source, const void* flow, const void* weight
                           accumulate, (cudaStream_t)stream);
 }
 
-// ------------------------------------------------------------------ deterministic backward passes (det_accum.cuh)
-// The workspace of each: the fixed-point sums of every scattered output, the exponents and the maxima (fx_layout).
-static FxLayout la_det_layout(int B, int C, int Hs, int Ws) { return fx_layout((long long)B * C * Hs * Ws, B, B); }
-static FxLayout be_det_layout(int B, int C, int Hs, int Ws) { return fx_layout((long long)B * C * Hs * Ws, B, B); }
-static FxLayout pc_det_layout(int B, int C, int Hs, int Ws, int k, int N) {
-    return fx_layout((long long)B * Hs * Ws * C + (long long)N * k * k * C, B + 1, B + 2);
-}
-
-// NULL workspace: GFLA_E_NULL; not 16-byte aligned: GFLA_E_ALIGN; smaller than needed: GFLA_E_SHAPE
-static int ws_check(const void* ws, long long bytes, const FxLayout& l) {
-    if (ws == nullptr) return GFLA_E_NULL;
-    if (!aligned(ws, 16)) return GFLA_E_ALIGN;
-    if (bytes < 0 || (size_t)bytes < l.total) return GFLA_E_SHAPE;
-    return GFLA_OK;
-}
-
-#define FX_PARTS(ws, l) \
-    fx_t* sums = reinterpret_cast<fx_t*>(ws); \
-    int* exps = reinterpret_cast<int*>(static_cast<char*>(ws) + (l).exps); \
-    fx_t* amax = reinterpret_cast<fx_t*>(static_cast<char*>(ws) + (l).amax)
-
+// ------------------------------------------------------------------ deterministic backward passes
 long long gfla_local_attn_bwd_det_workspace_bytes(int B, int C, int Hs, int Ws, int H, int W, int k) {
-    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || k < 1 || k > 9) return GFLA_E_SHAPE;
-    return (long long)la_det_layout(B, C, Hs, Ws).total;
+    if (!pos(B, C, Hs, Ws, H, W) || !k_ok(k)) return GFLA_E_SHAPE;
+    return (long long)scatter_det_layout(B, C, Hs, Ws).total;
 }
 
 int gfla_local_attn_bwd_det(const void* source, const void* flow, const void* logits, const void* grad_out, void* grad_source,
                             void* grad_flow, void* grad_logits, int B, int C, int Hs, int Ws, int H, int W, int k, int dtype,
                             int flow_dtype, int layout, int accumulate, int algo, void* workspace, long long workspace_bytes,
                             gfla_stream_t stream) {
-    if (layout != GFLA_NCHW && layout != GFLA_NHWC) return GFLA_E_SHAPE;
-    REQ_PTR(source); REQ_PTR(flow); REQ_PTR(logits); REQ_PTR(grad_out); REQ_PTR(grad_source); REQ_PTR(grad_flow); REQ_PTR(grad_logits);
-    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || k < 1 || k > 9) return GFLA_E_SHAPE;
-    if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
-    if (algo < 0 || algo > 2) return GFLA_E_NOTSUP;
-    REQ_ALIGN(source, dtype); REQ_ALIGN(logits, dtype); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_source, dtype);
-    REQ_ALIGN(grad_logits, dtype); REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
-    const FxLayout l = la_det_layout(B, C, Hs, Ws);
-    const int w = ws_check(workspace, workspace_bytes, l);
-    if (w != GFLA_OK) return w;
+    REQ_OK(local_attn_bwd_args(source, flow, logits, grad_out, grad_source, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype,
+                               flow_dtype, layout, algo));
+    const FxLayout l = scatter_det_layout(B, C, Hs, Ws);
+    REQ_OK(ws_check(workspace, workspace_bytes, l));
     // the tile kernel never writes grad_source here (fx_narrow does): its alignment must not change which kernel runs
     const bool tc_ok = local_attn_bwd_tc_supported(C, k, dtype, flow_dtype, layout, source, grad_out, source);
     if (algo == 2 && !tc_ok) return GFLA_E_NOTSUP;
+    const bool tile = algo == 2 || (algo == 0 && tc_ok);
     const cudaStream_t st_ = (cudaStream_t)stream;
-    FX_PARTS(workspace, l);
-    int r = zero_async(workspace, l.total, st_);
-    if (r == GFLA_OK) r = fx_amax(grad_out, dtype, (long long)C * H * W, B, amax, st_);
     // Bound of image b: every pixel spreads g_c times weights that sum to exactly 1/k^2 (softmax probabilities summing to
     // 1, times bilinear weights summing to 1, times 1/k^2) over the source positions, so every grad_source element of the
     // image is at most (H W / k^2) max|G_b| in magnitude, and so is the sum of the magnitudes of its partials.  The tile
@@ -377,53 +391,43 @@ int gfla_local_attn_bwd_det(const void* source, const void* flow, const void* lo
     // subnormal and off by at most 2^-25 absolutely, (k+1)^2 2^-25 per pixel at most: against the pixel's weight sum 1/k^2
     // that is k^2 (k+1)^2 2^-25 <= 900 2^-25 < 2^-15 (k <= 5, the only tile sizes).  Together below 1 + 2^-10.  Either
     // factor stays far inside the one bit of margin below 2^62 (det_accum.cuh), which only requires a factor below 2.
-    if (r == GFLA_OK) r = fx_exponents(amax, B, nullptr, (double)H * W / ((double)k * k), false, exps, st_);
-    if (r == GFLA_OK) {
-        if (algo == 2 || (algo == 0 && tc_ok))
-            r = local_attn_bwd_tc_det(source, flow, logits, grad_out, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype, accumulate,
-                                      sums, exps, st_);
-        else
-            r = local_attn_bwd_gather_det(source, flow, logits, grad_out, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype,
-                                          flow_dtype, accumulate, layout, sums, exps, st_);
-    }
-    if (r == GFLA_OK)
-        r = fx_narrow(sums, exps, (long long)C * Hs * Ws, (long long)B * C * Hs * Ws, grad_source, dtype, accumulate, st_);
-    return r;
+    return det_scatter(workspace, l, grad_out, (long long)C * H * W, (double)H * W / ((double)k * k), grad_source,
+                       (long long)C * Hs * Ws, B, dtype, accumulate, st_, [&](fx_t* sums, const int* exps) {
+        if (tile)
+            return local_attn_bwd_tc_det(source, flow, logits, grad_out, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype, accumulate,
+                                         sums, exps, st_);
+        return local_attn_bwd_gather_det(source, flow, logits, grad_out, grad_flow, grad_logits, B, C, Hs, Ws, H, W, k, dtype,
+                                         flow_dtype, accumulate, layout, sums, exps, st_);
+    });
 }
 
 long long gfla_block_extract_bwd_det_workspace_bytes(int B, int C, int Hs, int Ws, int Hf, int Wf, int k) {
-    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(Hf) || !pos(Wf) || k < 1 || k > 9) return GFLA_E_SHAPE;
-    return (long long)be_det_layout(B, C, Hs, Ws).total;
+    if (!pos(B, C, Hs, Ws, Hf, Wf) || !k_ok(k)) return GFLA_E_SHAPE;
+    return (long long)scatter_det_layout(B, C, Hs, Ws).total;
 }
 
 int gfla_block_extract_bwd_det(const void* source, const void* flow, const void* grad_out, void* grad_source, void* grad_flow,
                                int B, int C, int Hs, int Ws, int Hf, int Wf, int k, int dtype, int flow_dtype, int accumulate,
                                void* workspace, long long workspace_bytes, gfla_stream_t stream) {
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(grad_out); REQ_PTR(grad_source); REQ_PTR(grad_flow);
-    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(Hf) || !pos(Wf) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    if (!pos(B, C, Hs, Ws, Hf, Wf) || !k_ok(k)) return GFLA_E_SHAPE;
     if (!dtypes_ok(dtype, flow_dtype, dtype)) return GFLA_E_DTYPE;
     REQ_ALIGN(source, dtype); REQ_ALIGN(grad_out, dtype); REQ_ALIGN(grad_source, dtype);
     REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
-    const FxLayout l = be_det_layout(B, C, Hs, Ws);
-    const int w = ws_check(workspace, workspace_bytes, l);
-    if (w != GFLA_OK) return w;
+    const FxLayout l = scatter_det_layout(B, C, Hs, Ws);
+    REQ_OK(ws_check(workspace, workspace_bytes, l));
     const cudaStream_t st_ = (cudaStream_t)stream;
-    FX_PARTS(workspace, l);
-    int r = zero_async(workspace, l.total, st_);
-    if (r == GFLA_OK) r = fx_amax(grad_out, dtype, (long long)C * k * Hf * k * Wf, B, amax, st_);
     // Bound of image b: every grad_out element spreads bilinear weights that sum to 1 over 4 source positions of its
     // channel, so a grad_source element collects at most the k^2 Hf Wf elements of its channel: k^2 Hf Wf max|G_b|.
-    if (r == GFLA_OK) r = fx_exponents(amax, B, nullptr, (double)k * k * Hf * Wf, false, exps, st_);
-    if (r == GFLA_OK)
-        r = block_extract_bwd_det(source, flow, grad_out, grad_flow, B, C, Hs, Ws, Hf, Wf, k, dtype, flow_dtype, accumulate, sums, exps,
-                                  st_);
-    if (r == GFLA_OK)
-        r = fx_narrow(sums, exps, (long long)C * Hs * Ws, (long long)B * C * Hs * Ws, grad_source, dtype, accumulate, st_);
-    return r;
+    return det_scatter(workspace, l, grad_out, (long long)C * k * Hf * k * Wf, (double)k * k * Hf * Wf, grad_source,
+                       (long long)C * Hs * Ws, B, dtype, accumulate, st_, [&](fx_t* sums, const int* exps) {
+        return block_extract_bwd_det(source, flow, grad_out, grad_flow, B, C, Hs, Ws, Hf, Wf, k, dtype, flow_dtype, accumulate, sums,
+                                     exps, st_);
+    });
 }
 
 long long gfla_patch_conv_bwd_det_workspace_bytes(int B, int C, int Hs, int Ws, int H, int W, int k, int N) {
-    if (!pos(B) || !pos(C) || !pos(Hs) || !pos(Ws) || !pos(H) || !pos(W) || !pos(N) || k < 1 || k > 9) return GFLA_E_SHAPE;
+    if (!pos(B, C, Hs, Ws, H, W, N) || !k_ok(k)) return GFLA_E_SHAPE;
     return (long long)pc_det_layout(B, C, Hs, Ws, k, N).total;
 }
 
@@ -433,13 +437,11 @@ int gfla_patch_conv_bwd_det(const void* source, const void* flow, const void* we
                             gfla_stream_t stream) {
     REQ_PTR(source); REQ_PTR(flow); REQ_PTR(weight); REQ_PTR(grad_out);
     REQ_PTR(grad_source); REQ_PTR(grad_flow); REQ_PTR(grad_weight);
-    const int e = patch_conv_args(B, C, Hs, Ws, H, W, k, N, dtype, flow_dtype, layout);
-    if (e != GFLA_OK) return e;
+    REQ_OK(patch_conv_args(B, C, Hs, Ws, H, W, k, N, dtype, flow_dtype, layout));
     if (!aligned(source, 16) || !aligned(weight, 16) || !aligned(grad_out, 16)) return GFLA_E_ALIGN;
     REQ_ALIGN(grad_source, dtype); REQ_ALIGN(grad_weight, dtype); REQ_ALIGN(flow, flow_dtype); REQ_ALIGN(grad_flow, flow_dtype);
     const FxLayout l = pc_det_layout(B, C, Hs, Ws, k, N);
-    const int w = ws_check(workspace, workspace_bytes, l);
-    if (w != GFLA_OK) return w;
+    REQ_OK(ws_check(workspace, workspace_bytes, l));
     const cudaStream_t st_ = (cudaStream_t)stream;
     FX_PARTS(workspace, l);
     const long long n_src = (long long)B * Hs * Ws * C, n_w = (long long)N * k * k * C;
@@ -461,7 +463,7 @@ int gfla_patch_conv_bwd_det(const void* source, const void* flow, const void* we
     return r;
 }
 
-long long gfla_local_attn_bwd_workspace_bytes(int B) { (void)B; return 0; }   // the tile backward needs no workspace
+long long gfla_local_attn_bwd_workspace_bytes(int B) { (void)B; return 0; }   // the tile backward's scratch: the library's pool
 
 int gfla_local_attn_bwd_ws(const void* source, const void* flow, const void* logits, const void* grad_out,
                            void* grad_source, void* grad_flow, void* grad_logits, int B, int C, int Hs, int Ws, int H, int W,

@@ -559,6 +559,26 @@ static int pick_cn_bwd(int C) {
     return 0;
 }
 
+// the instance of k_local_attn_bwd_tc for (dtype, k, cn); GFLA_E_NOTSUP for a (k, cn) without one
+template <bool DET, typename T>
+static int dispatch_bwd_t(int k, int cn, const void* src, const void* flow, const void* logits, const void* gout, void* gsrc, void* gflow,
+                          void* glogits, float* gborder, int B, int C, int Hs, int Ws, int H, int W, int accumulate, cudaStream_t st_,
+                          fx_t* gsum, const int* fx_exp) {
+#define GFLA_BT_CASE(K_, CN_) \
+    if (k == K_ && cn == CN_) return tc::launch_bwd<K_, CN_, DET, T>(src, flow, logits, gout, gsrc, gflow, glogits, gborder, B, C, Hs, Ws, \
+                                                                     H, W, accumulate, st_, gsum, fx_exp);
+    GFLA_BT_CASE(5, 256) GFLA_BT_CASE(5, 128) GFLA_BT_CASE(5, 64)
+    GFLA_BT_CASE(3, 256) GFLA_BT_CASE(3, 128) GFLA_BT_CASE(3, 64)
+#undef GFLA_BT_CASE
+    return GFLA_E_NOTSUP;
+}
+
+template <bool DET, typename... A>
+static int dispatch_bwd(int k, int cn, int dtype, A... a) {
+    if (dtype == GFLA_F16) return dispatch_bwd_t<DET, __half>(k, cn, a...);
+    return dispatch_bwd_t<DET, __nv_bfloat16>(k, cn, a...);
+}
+
 bool local_attn_bwd_tc_supported(int C, int k, int dtype, int flow_dtype, int layout, const void* src, const void* gout,
                                  const void* gsrc) {
     return (dtype == GFLA_BF16 || dtype == GFLA_F16) && flow_dtype == GFLA_F32 && layout == GFLA_NHWC && (k == 3 || k == 5) && pick_cn_bwd(C) != 0 &&
@@ -581,18 +601,9 @@ int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, con
     cudaError_t e = scratch_alloc(reinterpret_cast<void**>(&gborder), border_bytes, st_);
     if (e != cudaSuccess) return static_cast<int>(e);
     int r = zero_async(gborder, border_bytes, st_);
-    if (r == GFLA_OK) {
-#define GFLA_BT_CASE(T_, K_, CN_) \
-        if (k == K_ && cn == CN_) r = tc::launch_bwd<K_, CN_, false, T_>(src, flow, logits, gout, gsrc, gflow, glogits, gborder, B, C, Hs, Ws, H, W, accumulate, st_);
-        if (dtype == GFLA_F16) {
-            GFLA_BT_CASE(__half, 5, 256) GFLA_BT_CASE(__half, 5, 128) GFLA_BT_CASE(__half, 5, 64)
-            GFLA_BT_CASE(__half, 3, 256) GFLA_BT_CASE(__half, 3, 128) GFLA_BT_CASE(__half, 3, 64)
-        } else {
-            GFLA_BT_CASE(__nv_bfloat16, 5, 256) GFLA_BT_CASE(__nv_bfloat16, 5, 128) GFLA_BT_CASE(__nv_bfloat16, 5, 64)
-            GFLA_BT_CASE(__nv_bfloat16, 3, 256) GFLA_BT_CASE(__nv_bfloat16, 3, 128) GFLA_BT_CASE(__nv_bfloat16, 3, 64)
-        }
-#undef GFLA_BT_CASE
-    }
+    if (r == GFLA_OK)
+        r = dispatch_bwd<false>(k, cn, dtype, src, flow, logits, gout, gsrc, gflow, glogits, gborder, B, C, Hs, Ws, H, W, accumulate, st_,
+                                nullptr, nullptr);
     e = cudaFreeAsync(gborder, st_);
     return r != GFLA_OK ? r : static_cast<int>(e);
 }
@@ -602,19 +613,8 @@ int local_attn_bwd_tc(const void* src, const void* flow, const void* logits, con
 int local_attn_bwd_tc_det(const void* src, const void* flow, const void* logits, const void* gout, void* gflow, void* glogits, int B,
                           int C, int Hs, int Ws, int H, int W, int k, int dtype, int accumulate, fx_t* gsum, const int* fx_exp,
                           cudaStream_t st_) {
-    const int cn = pick_cn_bwd(C);
-#define GFLA_BT_CASE(T_, K_, CN_) \
-    if (k == K_ && cn == CN_) return tc::launch_bwd<K_, CN_, true, T_>(src, flow, logits, gout, nullptr, gflow, glogits, nullptr, B, C, Hs, \
-                                                                       Ws, H, W, accumulate, st_, gsum, fx_exp);
-    if (dtype == GFLA_F16) {
-        GFLA_BT_CASE(__half, 5, 256) GFLA_BT_CASE(__half, 5, 128) GFLA_BT_CASE(__half, 5, 64)
-        GFLA_BT_CASE(__half, 3, 256) GFLA_BT_CASE(__half, 3, 128) GFLA_BT_CASE(__half, 3, 64)
-    } else {
-        GFLA_BT_CASE(__nv_bfloat16, 5, 256) GFLA_BT_CASE(__nv_bfloat16, 5, 128) GFLA_BT_CASE(__nv_bfloat16, 5, 64)
-        GFLA_BT_CASE(__nv_bfloat16, 3, 256) GFLA_BT_CASE(__nv_bfloat16, 3, 128) GFLA_BT_CASE(__nv_bfloat16, 3, 64)
-    }
-#undef GFLA_BT_CASE
-    return GFLA_E_NOTSUP;
+    return dispatch_bwd<true>(k, pick_cn_bwd(C), dtype, src, flow, logits, gout, nullptr, gflow, glogits, nullptr, B, C, Hs, Ws, H, W,
+                              accumulate, st_, gsum, fx_exp);
 }
 
 }  // namespace gfla

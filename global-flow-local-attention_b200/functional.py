@@ -66,6 +66,19 @@ def _p(t):
     return None if t is None else t.data_ptr()
 
 
+def _call(name: str, t: torch.Tensor, *args) -> None:
+    """Calls the entry point gfla_<name> with args on t's device and its current stream, and raises GflaError naming
+    `name` if the call fails."""
+    with torch.cuda.device_of(t):
+        _lib.check(getattr(_lib.lib(), "gfla_" + name)(*args, _stream(t)), name)
+
+
+def _resample2d_op(op: str, input1: torch.Tensor) -> str:
+    """the resample2d entry point `op` (fwd, cosine_fwd, ...) for input1's dtype: the resample2d16 family for 16-bit
+    feature maps, resample2d for fp32 / fp64"""
+    return ("resample2d16_" if input1.dtype in _HALF else "resample2d_") + op
+
+
 # --------------------------------------------------------------------------- deterministic mode
 def alert_not_deterministic(caller: str) -> None:
     """What PyTorch's ops do without a deterministic implementation: raise under torch.use_deterministic_algorithms(True),
@@ -110,6 +123,13 @@ def _workspace(nbytes: int, device) -> torch.Tensor:
         return torch.empty(nbytes, dtype=torch.uint8, device=device)
 
 
+def _call_det(name: str, t: torch.Tensor, sizes, *args) -> None:
+    """A *_det entry point: its workspace, sized by gfla_<name>_workspace_bytes(*sizes), is appended to args."""
+    nbytes = getattr(_lib.lib(), f"gfla_{name}_workspace_bytes")(*sizes)
+    wsp = _workspace(nbytes, t.device)
+    _call(name, t, *args, _p(wsp), nbytes)
+
+
 # --------------------------------------------------------------------------- block_extractor
 def block_extract_fwd(source: torch.Tensor, flow: torch.Tensor, k: int) -> torch.Tensor:
     assert source.is_contiguous() and flow.is_contiguous()
@@ -118,9 +138,7 @@ def block_extract_fwd(source: torch.Tensor, flow: torch.Tensor, k: int) -> torch
     assert df == 2
     _need_cuda(source, flow)
     out = source.new_empty((bs, ds, k * hf, k * wf))   # fully written by the kernel: no zero fill needed
-    with torch.cuda.device_of(source):
-        _lib.check(_lib.lib().gfla_block_extract_fwd(_p(source), _p(flow), _p(out), bs, ds, hs, ws, hf, wf, k,
-                                                     _dt(source), _dt(flow), _stream(source)), "block_extract_fwd")
+    _call("block_extract_fwd", source, _p(source), _p(flow), _p(out), bs, ds, hs, ws, hf, wf, k, _dt(source), _dt(flow))
     return out
 
 
@@ -128,8 +146,7 @@ def convert(t: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
     """fp32 <-> bf16/f16 copy with the library's kernel (contiguous tensors)."""
     assert t.is_contiguous()
     out = torch.empty_like(t, dtype=dtype)
-    with torch.cuda.device_of(t):
-        _lib.check(_lib.lib().gfla_convert(_p(t), _dt(t), _p(out), _DT[dtype], t.numel(), _stream(t)), "convert")
+    _call("convert", t, _p(t), _dt(t), _p(out), _DT[dtype], t.numel())
     return out
 
 
@@ -156,10 +173,8 @@ def block_extract_bwd(source, flow, grad_out, k, grad_source=None, grad_flow=Non
         if flow.dtype in (torch.bfloat16, torch.float16):
             flow_in = convert(flow, torch.float32)
         grad_flow = torch.empty_like(flow_in)
-    with torch.cuda.device_of(source):
-        _lib.check(_lib.lib().gfla_block_extract_bwd(_p(source), _p(flow_in), _p(grad_out), _p(grad_source), _p(grad_flow),
-                                                     bs, ds, hs, ws, hf, wf, k, _dt(source), _dt(flow_in), _dt(grad_source),
-                                                     accumulate, _stream(source)), "block_extract_bwd")
+    _call("block_extract_bwd", source, _p(source), _p(flow_in), _p(grad_out), _p(grad_source), _p(grad_flow), bs, ds, hs, ws,
+          hf, wf, k, _dt(source), _dt(flow_in), _dt(grad_source), accumulate)
     if narrow:
         grad_source = convert(grad_source, source.dtype)
     if flow_in is not flow:
@@ -181,13 +196,8 @@ def _block_extract_bwd_det(source, flow, grad_out, k, grad_source, grad_flow):
         # the sums are rounded once, into the source's (flow's) dtype: a wider buffer would only add a second rounding
         raise TypeError(f"deterministic block_extract backward: grad_source / grad_flow must have the dtypes of source / "
                         f"flow ({source.dtype} / {flow.dtype}), got {grad_source.dtype} / {grad_flow.dtype}")
-    l = _lib.lib()
-    nb = l.gfla_block_extract_bwd_det_workspace_bytes(bs, ds, hs, ws, hf, wf, k)
-    wsp = _workspace(nb, source.device)
-    with torch.cuda.device_of(source):
-        _lib.check(l.gfla_block_extract_bwd_det(_p(source), _p(flow), _p(grad_out), _p(grad_source), _p(grad_flow), bs, ds, hs, ws,
-                                                hf, wf, k, _dt(source), _dt(flow), accumulate, _p(wsp), nb, _stream(source)),
-                   "block_extract_bwd_det")
+    _call_det("block_extract_bwd_det", source, (bs, ds, hs, ws, hf, wf, k), _p(source), _p(flow), _p(grad_out), _p(grad_source),
+              _p(grad_flow), bs, ds, hs, ws, hf, wf, k, _dt(source), _dt(flow), accumulate)
     return grad_source, grad_flow
 
 
@@ -198,9 +208,7 @@ def attn_reshape_fwd(inputs: torch.Tensor, k: int) -> torch.Tensor:
     assert ds == k * k
     _need_cuda(inputs)
     out = inputs.new_empty((bs, 1, k * hs, k * ws))
-    with torch.cuda.device_of(inputs):
-        _lib.check(_lib.lib().gfla_attn_reshape_fwd(_p(inputs), _p(out), bs, hs, ws, k, _dt(inputs), _stream(inputs)),
-                   "attn_reshape_fwd")
+    _call("attn_reshape_fwd", inputs, _p(inputs), _p(out), bs, hs, ws, k, _dt(inputs))
     return out
 
 
@@ -212,9 +220,7 @@ def attn_reshape_bwd(grad_out: torch.Tensor, k: int, grad_in=None) -> torch.Tens
     accumulate = 1
     if grad_in is None:
         grad_in, accumulate = grad_out.new_empty((bs, k * k, hs, ws)), 0
-    with torch.cuda.device_of(grad_out):
-        _lib.check(_lib.lib().gfla_attn_reshape_bwd(_p(grad_out), _p(grad_in), bs, hs, ws, k, _dt(grad_out), accumulate,
-                                                    _stream(grad_out)), "attn_reshape_bwd")
+    _call("attn_reshape_bwd", grad_out, _p(grad_out), _p(grad_in), bs, hs, ws, k, _dt(grad_out), accumulate)
     return grad_in
 
 
@@ -230,10 +236,8 @@ def resample2d_fwd(input1: torch.Tensor, input2: torch.Tensor, kernel_size: int,
     if not half and input2.dtype != input1.dtype:
         raise TypeError("resample2d: input1 and input2 must share a dtype (float32 or float64)")
     out = input1.new_empty((b, d, h, w))
-    fn = _lib.lib().gfla_resample2d16_fwd if half else _lib.lib().gfla_resample2d_fwd
-    with torch.cuda.device_of(input1):
-        _lib.check(fn(_p(input1), _p(input2), _p(out), b, d, hi, wi, h, w, kernel_size, dilation, _dt(input1), _stream(input1)),
-                   "resample2d_fwd")
+    _call(_resample2d_op("fwd", input1), input1, _p(input1), _p(input2), _p(out), b, d, hi, wi, h, w, kernel_size, dilation,
+          _dt(input1))
     return out
 
 
@@ -254,17 +258,14 @@ def resample2d_bwd(input1, input2, grad_out, kernel_size, dilation, grad_input1=
             raise TypeError(f"resample2d backward: grad_out must have input1's dtype {input1.dtype}, got {grad_out.dtype}")
         gin1 = torch.empty(input1.shape, dtype=torch.float32, device=input1.device)
         gin2 = torch.empty_like(input2)
-        with torch.cuda.device_of(input1):
-            _lib.check(_lib.lib().gfla_resample2d16_bwd(_p(input1), _p(input2), _p(grad_out), _p(gin1), _p(gin2), b, d, hi, wi, h, w,
-                                                        kernel_size, dilation, _dt(input1), 0, _stream(input1)), "resample2d_bwd")
+        _call("resample2d16_bwd", input1, _p(input1), _p(input2), _p(grad_out), _p(gin1), _p(gin2), b, d, hi, wi, h, w,
+              kernel_size, dilation, _dt(input1), 0)
         return convert(gin1, input1.dtype), gin2
     accumulate = 1
     if grad_input1 is None:
         grad_input1, grad_input2, accumulate = torch.empty_like(input1), torch.empty_like(input2), 0
-    with torch.cuda.device_of(input1):
-        _lib.check(_lib.lib().gfla_resample2d_bwd(_p(input1), _p(input2), _p(grad_out), _p(grad_input1), _p(grad_input2),
-                                                  b, d, hi, wi, h, w, kernel_size, dilation, _dt(input1), accumulate,
-                                                  _stream(input1)), "resample2d_bwd")
+    _call("resample2d_bwd", input1, _p(input1), _p(input2), _p(grad_out), _p(grad_input1), _p(grad_input2), b, d, hi, wi, h, w,
+          kernel_size, dilation, _dt(input1), accumulate)
     return grad_input1, grad_input2
 
 
@@ -285,10 +286,8 @@ def resample2d_cosine_fwd(input1, input2, target, kernel_size: int, dilation: in
                         "target a 16-bit one")
     cos = input1.new_empty((b, h, w))
     stats = input2.new_empty((b, 3, h, w))
-    fn = _lib.lib().gfla_resample2d16_cosine_fwd if half else _lib.lib().gfla_resample2d_cosine_fwd
-    with torch.cuda.device_of(input1):
-        _lib.check(fn(_p(input1), _p(input2), _p(target), _p(cos), _p(stats), b, d, hi, wi, h, w, kernel_size, dilation, float(eps),
-                      _dt(input1), _stream(input1)), "resample2d_cosine_fwd")
+    _call(_resample2d_op("cosine_fwd", input1), input1, _p(input1), _p(input2), _p(target), _p(cos), _p(stats), b, d, hi, wi, h, w,
+          kernel_size, dilation, float(eps), _dt(input1))
     return cos, stats
 
 
@@ -312,12 +311,8 @@ def resample2d_cosine_bwd(input1, input2, target, stats, grad_cos, kernel_size, 
     grad_in1 = torch.empty_like(input1, dtype=wide) if need_input1 else None
     grad_val = torch.empty_like(target, dtype=wide) if need_input1 else None
     grad_target = torch.empty_like(target) if need_target else None
-    fn = _lib.lib().gfla_resample2d16_cosine_bwd if half else _lib.lib().gfla_resample2d_cosine_bwd
-    with torch.cuda.device_of(input1):
-        _lib.check(fn(
-            _p(input1), _p(input2), _p(target), _p(stats), _p(grad_cos), _p(grad_in1) if need_input1 else None, _p(grad_in2),
-            _p(grad_val) if need_input1 else None, _p(grad_target) if need_target else None, b, d, hi, wi, h, w, kernel_size, dilation,
-            float(eps), _dt(input1), 0, _stream(input1)), "resample2d_cosine_bwd")
+    _call(_resample2d_op("cosine_bwd", input1), input1, _p(input1), _p(input2), _p(target), _p(stats), _p(grad_cos), _p(grad_in1),
+          _p(grad_in2), _p(grad_val), _p(grad_target), b, d, hi, wi, h, w, kernel_size, dilation, float(eps), _dt(input1), 0)
     if half and need_input1:
         del grad_val
         grad_in1 = convert(grad_in1, input1.dtype)
@@ -353,10 +348,8 @@ def local_attn_fwd(source, flow, logits, k, return_probs=False, algo="auto"):
     assert logits.shape == (bs, k * k, h, w) and logits.dtype == source.dtype
     out = _like_layout(source, (bs, ds, h, w), layout)
     probs = torch.empty_like(logits) if return_probs else None
-    with torch.cuda.device_of(source):
-        _lib.check(_lib.lib().gfla_local_attn_fwd(_p(source), _p(flow), _p(logits), _p(out), _p(probs), bs, ds, hs, ws,
-                                                  h, w, k, _dt(source), _dt(flow), layout, ALGO[algo], _stream(source)),
-                   "local_attn_fwd")
+    _call("local_attn_fwd", source, _p(source), _p(flow), _p(logits), _p(out), _p(probs), bs, ds, hs, ws, h, w, k, _dt(source),
+          _dt(flow), layout, ALGO[algo])
     return (out, probs) if return_probs else out
 
 
@@ -373,10 +366,8 @@ def local_attn_blend_fwd(source, flow, logits, prev, mask, k, algo="auto"):
     assert prev.shape == (bs, ds, h, w) and mask.shape == (bs, 1, h, w)
     assert prev.dtype == source.dtype and mask.dtype == source.dtype and logits.dtype == source.dtype
     out = _like_layout(source, (bs, ds, h, w), layout)
-    with torch.cuda.device_of(source):
-        _lib.check(_lib.lib().gfla_local_attn_blend_fwd(_p(source), _p(flow), _p(logits), _p(prev), _p(mask), _p(out), bs, ds,
-                                                        hs, ws, h, w, k, _dt(source), _dt(flow), layout, ALGO[algo],
-                                                        _stream(source)), "local_attn_blend_fwd")
+    _call("local_attn_blend_fwd", source, _p(source), _p(flow), _p(logits), _p(prev), _p(mask), _p(out), bs, ds, hs, ws, h, w, k,
+          _dt(source), _dt(flow), layout, ALGO[algo])
     return out
 
 
@@ -390,9 +381,7 @@ def relayout(t: torch.Tensor, to_channels_last: bool) -> torch.Tensor:
     else:
         assert t.is_contiguous(memory_format=torch.channels_last)
         out = torch.empty((b, c, h, w), dtype=t.dtype, device=t.device)
-    with torch.cuda.device_of(t):
-        _lib.check(_lib.lib().gfla_relayout(_p(t), _p(out), b, c, h, w, _dt(t), 1 if to_channels_last else 0, _stream(t)),
-                   "relayout")
+    _call("relayout", t, _p(t), _p(out), b, c, h, w, _dt(t), 1 if to_channels_last else 0)
     return out
 
 
@@ -426,9 +415,8 @@ def patch_conv_fwd(source, flow, weight, k):
     n = weight.shape[0]
     wp = _pack_weight(weight)
     out = torch.empty((bs, h, w, n), dtype=source.dtype, device=source.device)       # channels-last storage
-    with torch.cuda.device_of(source):
-        _lib.check(_lib.lib().gfla_patch_conv_fwd(_p(src), _p(flow), _p(wp), _p(out), bs, ds, hs, ws, h, w, k, n, _dt(source),
-                                                  _dt(flow), _lib.GFLA_NHWC, _stream(source)), "patch_conv_fwd")
+    _call("patch_conv_fwd", source, _p(src), _p(flow), _p(wp), _p(out), bs, ds, hs, ws, h, w, k, n, _dt(source), _dt(flow),
+          _lib.GFLA_NHWC)
     out = out.permute(0, 3, 1, 2)
     return relayout(out, False) if planar else out
 
@@ -454,23 +442,15 @@ def patch_conv_bwd(source, flow, weight, grad_out, k):
             gs = torch.empty((bs, hs, ws, ds), dtype=source.dtype, device=source.device)   # channels-last storage
             gw = torch.empty((n, k, k, ds), dtype=weight.dtype, device=source.device)
             gf = torch.empty_like(flow)
-        l = _lib.lib()
-        nb = l.gfla_patch_conv_bwd_det_workspace_bytes(bs, ds, hs, ws, h, w, k, n)
-        wsp = _workspace(nb, source.device)
-        with torch.cuda.device_of(source):
-            _lib.check(l.gfla_patch_conv_bwd_det(_p(src), _p(flow), _p(wp), _p(go), _p(gs), _p(gf), _p(gw), bs, ds, hs, ws, h, w, k, n,
-                                                 _dt(source), _dt(flow), _lib.GFLA_NHWC, 0, _p(wsp), nb, _stream(source)),
-                       "patch_conv_bwd_det")
-        del wsp
+        _call_det("patch_conv_bwd_det", source, (bs, ds, hs, ws, h, w, k, n), _p(src), _p(flow), _p(wp), _p(go), _p(gs), _p(gf),
+                  _p(gw), bs, ds, hs, ws, h, w, k, n, _dt(source), _dt(flow), _lib.GFLA_NHWC, 0)
         gs, gw = gs.permute(0, 3, 1, 2), gw.permute(0, 3, 1, 2)
         return (relayout(gs, False) if planar else gs), gf, gw
     gs32 = torch.empty((bs, hs, ws, ds), dtype=torch.float32, device=source.device)   # channels-last storage
     gw32 = torch.empty((n, k, k, ds), dtype=torch.float32, device=source.device)
     gf = torch.empty_like(flow)
-    with torch.cuda.device_of(source):
-        _lib.check(_lib.lib().gfla_patch_conv_bwd(_p(src), _p(flow), _p(wp), _p(go), _p(gs32), _p(gf), _p(gw32), bs, ds, hs, ws,
-                                                  h, w, k, n, _dt(source), _dt(flow), _lib.GFLA_NHWC, 0, _stream(source)),
-                   "patch_conv_bwd")
+    _call("patch_conv_bwd", source, _p(src), _p(flow), _p(wp), _p(go), _p(gs32), _p(gf), _p(gw32), bs, ds, hs, ws, h, w, k, n,
+          _dt(source), _dt(flow), _lib.GFLA_NHWC, 0)
     gs = convert(gs32, source.dtype).permute(0, 3, 1, 2)
     del gs32
     gw = convert(gw32, weight.dtype).permute(0, 3, 1, 2)
@@ -510,10 +490,8 @@ def local_attn_bwd(source, flow, logits, grad_out, k, algo="auto"):
     bs, ds, hs, ws = source.size()
     _, _, h, w = flow.size()
     gs, gf, gl = _like_layout(source, source.shape, layout), torch.empty_like(flow), torch.empty_like(logits)
-    with torch.cuda.device_of(source):
-        _lib.check(_lib.lib().gfla_local_attn_bwd(_p(source), _p(flow), _p(logits), _p(grad_out), _p(gs), _p(gf), _p(gl),
-                                                  bs, ds, hs, ws, h, w, k, _dt(source), _dt(flow), layout, 0, ALGO[algo],
-                                                  _stream(source)), "local_attn_bwd")
+    _call("local_attn_bwd", source, _p(source), _p(flow), _p(logits), _p(grad_out), _p(gs), _p(gf), _p(gl), bs, ds, hs, ws, h, w,
+          k, _dt(source), _dt(flow), layout, 0, ALGO[algo])
     return gs, gf, gl
 
 
@@ -524,11 +502,6 @@ def _local_attn_bwd_det(source, flow, logits, grad_out, k, layout, algo):
     _, _, h, w = flow.size()
     with _no_fill():
         gs, gf, gl = _like_layout(source, source.shape, layout), torch.empty_like(flow), torch.empty_like(logits)
-    l = _lib.lib()
-    nb = l.gfla_local_attn_bwd_det_workspace_bytes(bs, ds, hs, ws, h, w, k)
-    wsp = _workspace(nb, source.device)
-    with torch.cuda.device_of(source):
-        _lib.check(l.gfla_local_attn_bwd_det(_p(source), _p(flow), _p(logits), _p(grad_out), _p(gs), _p(gf), _p(gl), bs, ds, hs, ws, h,
-                                             w, k, _dt(source), _dt(flow), layout, 0, ALGO[algo], _p(wsp), nb, _stream(source)),
-                   "local_attn_bwd_det")
+    _call_det("local_attn_bwd_det", source, (bs, ds, hs, ws, h, w, k), _p(source), _p(flow), _p(logits), _p(grad_out), _p(gs),
+              _p(gf), _p(gl), bs, ds, hs, ws, h, w, k, _dt(source), _dt(flow), layout, 0, ALGO[algo])
     return gs, gf, gl

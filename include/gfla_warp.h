@@ -15,8 +15,13 @@
  *   - `stream` is a cudaStream_t passed as void* (0 = legacy default stream).
  *     The reference launches on at::cuda::getCurrentCUDAStream()
  *     (block_extractor_kernel.cu:197); callers pass that same stream.
- *   - nothing is allocated, retained or synchronised inside the library; there
- *     is no global mutable state (safe under one host thread per GPU).
+ *   - nothing is synchronised inside the library.  It allocates in one place:
+ *     the tile backward (gfla_local_attn_bwd, gfla_local_attn_bwd_ws) takes
+ *     fp32 border sums, 2*(Hs+Ws)*C floats per image, stream-ordered from a
+ *     memory pool that the library creates for each device on first use and
+ *     keeps for the life of the process; the call hands them back to the pool
+ *     on its stream.  The only other state is a process-wide launch counter
+ *     (gfla_debug_launch_count).  Both are thread-safe.
  *   - return value: 0 on success; a negative GFLA_E_* code for argument
  *     errors (nothing was launched); a positive cudaError_t if a launch
  *     failed.  (The reference returns the constant 1 and checks nothing,
@@ -241,8 +246,8 @@ int gfla_local_attn_bwd(const void* source, const void* flow, const void* logits
                         int dtype, int flow_dtype, int layout, int accumulate, int algo,
                         gfla_stream_t stream);
 /* The same backward with a caller-provided scratch buffer (DEVICE memory, >= gfla_local_attn_bwd_workspace_bytes(B) bytes).
- * The current kernels need no scratch: the size is 0, the buffer is ignored and the call behaves exactly like
- * gfla_local_attn_bwd.  Kept so that callers written against ABI version 1 keep linking. */
+ * The size is 0, the buffer is ignored and the call behaves exactly like gfla_local_attn_bwd, whose tile kernel takes its
+ * scratch from the library's own pool (see Conventions).  Kept so that callers written against ABI version 1 keep linking. */
 long long gfla_local_attn_bwd_workspace_bytes(int B);
 int gfla_local_attn_bwd_ws(const void* source, const void* flow, const void* logits,
                            const void* grad_out,

@@ -307,6 +307,33 @@ def test_legacy_pybind_surface(oracle_lib):
     np.testing.assert_allclose(host(o2), oracle_lib.resample2d_fwd(s, host(in2), 2, 1), rtol=1e-6, atol=1e-6)
 
 
+def test_legacy_forwards_run_on_the_tensors_device():
+    """the shim's forwards launch on the device that holds their tensors, whichever device is current"""
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs two CUDA devices")
+    import gfla_b200
+    gfla_b200.compat.install()
+    import block_extractor_cuda, local_attn_reshape_cuda, resample2d_cuda  # noqa: E401
+    d1 = torch.device("cuda:1")
+    g = torch.Generator().manual_seed(12)
+    ts = torch.randn(1, 4, 10, 10, generator=g).to(d1)
+    tf = (torch.rand(1, 2, 10, 10, generator=g) * 8 - 4).to(d1)
+    x = torch.randn(1, 9, 5, 5, generator=g).to(d1)
+    in2 = torch.cat([tf, torch.full((1, 1, 10, 10), 5.0, device=d1)], 1)
+
+    def run(current):
+        with torch.cuda.device(current):
+            outs = (ts.new_zeros(1, 4, 30, 30), x.new_zeros(1, 1, 15, 15), ts.new_zeros(1, 4, 10, 10))
+            assert block_extractor_cuda.forward(ts, tf, outs[0], 3) == 1
+            assert local_attn_reshape_cuda.forward(x, outs[1], 3) == 1
+            assert resample2d_cuda.forward(ts, in2, outs[2], 2, 1) == 1
+        torch.cuda.synchronize(d1)
+        return outs
+
+    for a, b in zip(run(0), run(1)):
+        assert torch.equal(a, b)
+
+
 # ----------------------------------------------------------------------------- full-size properties (BASELINE cfg2 / cfg3)
 def _smooth_flow_t(B, H, W, amp=8.0, cell=16):
     coarse = (torch.rand(B, 2, H // cell, W // cell, device=DEV) * 2 - 1) * amp
